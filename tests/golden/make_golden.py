@@ -10,7 +10,8 @@ toggle / PutNext / Before / After paths of the verifier are exercised.
 
 usage: python tests/golden/make_golden.py [--only-missing] [--success]
        BABYAI_DONE_ACTIONS=1 python tests/golden/make_golden.py --done-actions
-       python tests/golden/make_golden.py --bonus [--only-missing]
+       python tests/golden/make_golden.py --bonus [--only-missing] [LEVEL ...]
+       BABYAI_DONE_ACTIONS=1 python tests/golden/make_golden.py --done-actions --bonus [LEVEL ...]
 """
 import json
 import os
@@ -128,28 +129,68 @@ def main_done():
               % (level, K, T, eps, succ, os.path.basename(out), os.path.getsize(out) // 1024), flush=True)
 
 
+def max_steps(level, episodes=64):
+    """the longest time limit among a level's first episodes (RoomGridLevel sets it per mission: one room-to-room
+    navigation budget per navigation the instruction needs)"""
+    env = refenv.make_env(level, 0, 'philox')
+    return max(env.reset() and env.max_steps for _ in range(episodes))
+
+
+def save_checked(out, level, seeds, tr):
+    """every trace must end at least one episode, so that the reset / ring swap-in path of every level is replayed"""
+    eps = [int(t['done'].sum()) for t in tr]
+    assert min(eps) > 0, (level, 'traces without an episode end', eps)
+    save(out, seeds, tr)
+    succ = sum(int((t['reward'] > 0).sum()) for t in tr)
+    print('%24s  %d traces x %d steps, %d episodes (%d successes, per trace %d..%d) -> %s (%d KB)'
+          % (level, len(tr), len(tr[0]['actions']), sum(eps), succ, min(eps), max(eps), os.path.basename(out),
+             os.path.getsize(out) // 1024), flush=True)
+
+
+BONUS_TRACES = 16
+
+
+def _selected(levels):
+    """the levels named on the command line (so that levels can be generated by parallel processes), else all"""
+    named = [a for a in sys.argv[1:] if not a.startswith('--')]
+    return [lv for lv in levels if lv in named] if named else levels
+
+
 def main_bonus():
-    """the 50 levels of babyai/levels/bonus_levels.py: 3 traces x 300 steps each, 60 % bot / 40 % random actions (random only
-    where the reference's bot does not return)"""
+    """the 50 levels of babyai/levels/bonus_levels.py: 16 traces each, 60 % bot / 40 % random actions (random only where the
+    reference's bot does not return).  Every trace is longer than the level's longest time limit (max_steps), so every trace
+    ends at least one episode even where only the time limit ends them (UnlockToUnlock, KeyInBox); save_checked asserts it."""
     sys.path.insert(0, ROOT)
     from babyai_b200.levels import BONUS_LEVELS
     only_missing = '--only-missing' in sys.argv
-    for level in BONUS_LEVELS:
+    for level in _selected(BONUS_LEVELS):
         out = os.path.join(HERE, 'bonus_' + level + '.npz')
         if only_missing and os.path.exists(out):
             continue
-        K, T = 3, 300
+        K, T = BONUS_TRACES, max(300, max_steps(level) + 40)
         seeds = [2000 + 11 * k for k in range(K)]
         p_bot = 0.0 if level in ('UnlockToUnlock', 'KeyInBox') else 0.6
-        tr = [trace(level, s, T, act_seed=500 + k, p_bot=p_bot) for k, s in enumerate(seeds)]
-        save(out, seeds, tr)
-        eps = sum(int(t['done'].sum()) for t in tr)
-        succ = sum(int((t['reward'] > 0).sum()) for t in tr)
-        print('%24s  %d traces x %d steps, %d episodes (%d successes) -> %s (%d KB)'
-              % (level, K, T, eps, succ, os.path.basename(out), os.path.getsize(out) // 1024), flush=True)
+        save_checked(out, level, seeds, [trace(level, s, T, act_seed=500 + k, p_bot=p_bot) for k, s in enumerate(seeds)])
+
+
+# done-action mode on bonus levels of every family: strict "Debug" verifiers (one of them single-room), the ordered
+# OpenDoorsOrder verifier, start-carrying PutNext, KeyCorridor and MoveTwoAcross
+DONE_BONUS_LEVELS = ['PickupDistDebug', 'OpenDoorsOrderN2Debug', 'OpenDoorsOrderN4', 'PutNextS6N3Carrying', 'KeyCorridorS3R3',
+                     'MoveTwoAcrossS5N2']
+
+
+def main_done_bonus():
+    assert os.environ.get('BABYAI_DONE_ACTIONS'), 'run with BABYAI_DONE_ACTIONS=1'
+    for level in _selected(DONE_BONUS_LEVELS):
+        out = os.path.join(HERE, 'done_bonus_' + level + '.npz')
+        K, T = BONUS_TRACES, 300
+        seeds = [3000 + 13 * k for k in range(K)]
+        save_checked(out, level, seeds, [trace(level, s, T, act_seed=700 + k, p_bot=0.8, p_done=0.03) for k, s in enumerate(seeds)])
 
 
 def main():
+    if '--done-actions' in sys.argv and '--bonus' in sys.argv:
+        return main_done_bonus()
     if '--bonus' in sys.argv:
         return main_bonus()
     if '--success' in sys.argv:

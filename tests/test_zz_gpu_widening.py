@@ -1,6 +1,7 @@
-"""GPU tests added after the last GPU visit of round 1 (the GPU budget was spent): they sort after
-test_gpu_parity.py so that `-x` reaches them last.  Their logic is exercised in the GPU-less suite through the host
-build of the kernel source (test_hostemu.py, test_learner_adapters.py); here the CUDA pool itself is on the other end."""
+"""GPU tests of the golden files test_gpu_parity.py does not replay, the device-resident learner adapters, the bench's own
+JSON line, the levels served by k_gen<true> and the C5 per-GPU share.  Their logic is also exercised in the GPU-less suite
+through the host build of the kernel source (test_hostemu.py, test_learner_adapters.py); here the CUDA pool itself is on the
+other end.  test_gpu_rollout_parity.py replays every golden file through bb_pool_rollout."""
 import numpy as np
 import pytest
 
