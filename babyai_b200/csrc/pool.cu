@@ -8,6 +8,7 @@
 //                 smaller than 6x6): one lane per environment, the warp in lock-step through one attempt per round.
 //   k_gen         level generation for every other level: one warp per level (generate_level).
 //   k_seed        env.seed().
+//   k_render_rgb, k_render_grid  pictures: the partial view of an observation, and the full grid of an env's current state.
 // Levels depend only on the env's random stream, never on actions, so generating episodes k+1 .. k+D while episode k
 // is being played is equivalent to generating them at reset time: every env owns a ring of D pre-generated levels.
 // The per-environment logic (step, verifier, observation, generators) is env_logic.cuh; DESIGN.md section 4 has the
@@ -31,6 +32,7 @@
 #include "step8.cuh"
 #include <type_traits>
 #include "rgb_tiles.h"
+#include "grid_render.cuh"
 
 using namespace bb;
 
@@ -402,6 +404,92 @@ k_render_rgb(const uint8_t *__restrict__ obs, uint8_t *__restrict__ rgb, const u
     }
 }
 
+// k_render_grid -- MiniGridEnv.render('rgb_array', highlight, tile_size) for selected envs: uint8[n_sel][H ts][W ts][3].
+// A frame is a pure function of the env's current state in HBM (grid bytes, pose) and of the table of 430 tiles
+// (rgb_tiles.h, render_grid_tiles) for the tile size: up to 484 grid bytes in, up to 5.9 MB (22 x 22 cells at 64 px) out,
+// so the kernel is bound by its stores.  One CTA per frame at a time (grid-stride over the selection):
+//   1. thread 0 reads the pose and computes the view's visibility (grid_render.cuh: col_load / col_see / vis_rows);
+//   2. every thread turns cells into tile offsets in shared memory (grid_tile_id, <= 484 cells; grid_hidden_cell: the object a
+//      PutNext*Carrying episode starts carrying is off the grid in the reference's state after reset);
+//   3. the CTA streams the frame out as V-byte pieces of tile rows: consecutive threads write consecutive pieces (coalesced
+//      streaming stores), each piece one load from the L2-resident table.  V = min(16, lowest set bit of ts) divides the tile
+//      row (3 ts bytes) and hence the frame, so a piece never straddles a tile and every frame of the 16-byte-aligned output
+//      starts V-aligned: 16-byte stores at ts 16 / 32 / 48 / 64, 8 at ts 8, single bytes at odd sizes (exact for every ts).
+// Where a piece comes from: the (tile column, offset in the tile row) of piece j of a pixel row is the same for every row and
+// env (s_pos, once per CTA); each thread walks its pieces with a fixed stride, so the pixel row / tile row it is in is
+// advanced by additions -- the loop has no division.
+constexpr int RG_THREADS = 256, RG_BLOCKS_PER_SM = 8, RG_IDS = 4096;
+
+// which envs a launch renders: frame k of the launch is env first + k (all envs, in order) or id[k] (a list of up to RG_IDS,
+// passed by value in the launch parameters: no device buffer, so calls on different streams share nothing)
+struct RgRange { int32_t first; __device__ __forceinline__ int env(int k) const { return first + k; } };
+struct RgList { int32_t id[RG_IDS]; __device__ __forceinline__ int env(int k) const { return id[k]; } };
+
+template <int V> struct RgVec;
+template <> struct RgVec<16> { typedef uint4 T; };
+template <> struct RgVec<8> { typedef uint2 T; };
+template <> struct RgVec<4> { typedef unsigned int T; };
+template <> struct RgVec<2> { typedef unsigned short T; };
+template <> struct RgVec<1> { typedef unsigned char T; };
+
+template <int V, class Sel>
+__global__ void __launch_bounds__(RG_THREADS)
+k_render_grid(const LevelParams lp, const PoolPtrs P, const Sel sel, const int n_sel, uint8_t *__restrict__ out,
+              const uint8_t *__restrict__ lut, const int ts, const int highlight)
+{
+    typedef typename RgVec<V>::T VT;
+    extern __shared__ __align__(16) uint32_t s_rg[];
+    __shared__ uint64_t s_vis;
+    __shared__ int s_pose, s_hidden;
+    const int W = lp.W, HW = lp.H * lp.W;
+    const int tile_row = 3 * ts, tile_bytes = tile_row * ts;
+    const int ppr = W * tile_row / V;                                  // pieces per pixel row
+    const uint32_t total = (uint32_t)(lp.H * ts) * (uint32_t)ppr;      // pieces per frame
+    const size_t frame_bytes = (size_t)total * V;
+    uint32_t *s_off = s_rg;                                            // [HW] table byte offset of each cell's tile
+    uint16_t *s_pos = reinterpret_cast<uint16_t *>(s_rg + HW);         // [ppr] tile column | byte offset in the tile row << 8
+    for (int j = threadIdx.x; j < ppr; j += RG_THREADS) {
+        const int c = j * V, tx = c / tile_row;
+        s_pos[j] = (uint16_t)(tx | ((c - tx * tile_row) << 8));
+    }
+    // this thread's first piece (pixel row r0 = tile row cy0, row ty0 inside it; piece j0) and the stride in the same terms
+    const int r0 = threadIdx.x / ppr, j0 = threadIdx.x - r0 * ppr;
+    const int cy0 = r0 / ts, ty0 = r0 - cy0 * ts;
+    const int dR = RG_THREADS / ppr, dJ = RG_THREADS - dR * ppr;
+    const int dCy = dR / ts, dTy = dR - dCy * ts;
+    for (int k = blockIdx.x; k < n_sel; k += gridDim.x) {
+        const int env = sel.env(k);
+        const uint8_t *grid = P.grid + (size_t)env * lp.cells_pad;
+        if (threadIdx.x == 0) {
+            const EnvHot h = P.hot[env];
+            const int dir = h.dirflags & 3;
+            s_pose = h.x | (h.y << 8) | (dir << 16);
+            s_vis = grid_view_vis(lp, GridWords{ grid }, h.x, h.y, dir);
+            s_hidden = lp.bonus == BN_PUTNEXT ? grid_hidden_cell(lp, h, P.obj[env], P.ins[env]) : -1;
+        }
+        __syncthreads();                          // (also: every thread is done with the previous frame's s_off)
+        const int pose = s_pose, ax = pose & 0xFF, ay = (pose >> 8) & 0xFF, dir = pose >> 16;
+        const uint64_t vis = s_vis;
+        const int hidden = s_hidden;
+        for (int c = threadIdx.x; c < HW; c += RG_THREADS) {
+            const int y = c / W, x = c - y * W;
+            const int cell = c == hidden ? CELL_EMPTY : grid[y * lp.rs_g + x];
+            s_off[c] = (uint32_t)grid_tile_id(cell, x, y, ax, ay, dir, vis, highlight != 0) * (uint32_t)tile_bytes;
+        }
+        __syncthreads();                          // (also: thread 0 may overwrite s_vis / s_pose for the next frame)
+        uint8_t *dst = out + (size_t)k * frame_bytes;
+        int j = j0, ty = ty0, cyw = cy0 * W;
+        for (uint32_t i = threadIdx.x; i < total; i += RG_THREADS) {
+            const uint32_t pos = s_pos[j];
+            const uint32_t src = s_off[cyw + (pos & 0xFF)] + (uint32_t)(ty * tile_row) + (pos >> 8);
+            __stcs(reinterpret_cast<VT *>(dst + (size_t)i * V), __ldg(reinterpret_cast<const VT *>(lut + src)));
+            j += dJ; ty += dTy; cyw += dCy * W;
+            if (j >= ppr) { j -= ppr; ty++; }
+            if (ty >= ts) { ty -= ts; cyw += W; }
+        }
+    }
+}
+
 __global__ void k_seed(const PoolPtrs P, const uint64_t *seeds, const int n)
 {
     const int env = blockIdx.x * blockDim.x + threadIdx.x;
@@ -454,6 +542,7 @@ struct bb_pool {
     // host-buffer API staging
     int8_t *h_act; uint8_t *h_obs; float *h_rew; uint8_t *h_done; int8_t *h_dir;      // pinned
     uint8_t *d_rgb_lut;            // the 513 RGB tiles (rgb_tiles.h), rendered on first use
+    uint8_t *d_grid_lut[bb_rgb::MAX_TILE_SIZE + 1];   // full-grid tile tables by tile size (rgb_tiles.h render_grid_tiles), rendered on first use
     int *h_err;                    // mapped: PoolPtrs::err_flag (a kernel found a level ring dry)
     int chain_cap;                 // BB_GEN_CHAIN_CAP: levels per env and pass of k_gen while the ring is at least half full (0 = no cap)
     int last_T, refill_cap;        // rollout length of the previous bb_pool_rollout call; BB_REFILL_EVERY as a cap for concurrent passes
@@ -593,6 +682,47 @@ static int sched_leave_rollout(bb_pool *p, cudaStream_t st)
     if (p->mode == BB_MODE_AUTORESET) launch_gen(p, st);
     p->after_rollout = false;
     return 0;
+}
+
+// the device table of one tile size: rasterised on the host and uploaded on first use (through the pool's internal stream,
+// which only the pool's synchronous entry points use), kept until bb_pool_destroy
+static int grid_table(bb_pool *p, int ts, const uint8_t **lut)
+{
+    if (!p->d_grid_lut[ts]) {
+        std::vector<uint8_t> h((size_t)bb_rgb::GRID_TILES * ts * ts * 3);
+        bb_rgb::render_grid_tiles(ts, h.data());
+        void *d = nullptr;
+        CU(cudaMalloc(&d, h.size()));
+        p->allocs.push_back(d);
+        CU(cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, p->stream));
+        CU(cudaStreamSynchronize(p->stream));
+        p->d_grid_lut[ts] = (uint8_t *)d;
+    }
+    *lut = p->d_grid_lut[ts];
+    return 0;
+}
+
+template <int V>
+static void launch_render_grid(bb_pool *p, const int32_t *ids, int32_t n_sel, int ts, int highlight, uint8_t *rgb, cudaStream_t st,
+                               const uint8_t *lut)
+{
+    const LevelParams &lp = p->lp;
+    const size_t frame = (size_t)lp.H * lp.W * ts * ts * 3;
+    const size_t smem = (size_t)lp.H * lp.W * 4 + (size_t)(lp.W * 3 * ts / V) * 2;
+    const int cap = p->sm_count * RG_BLOCKS_PER_SM;
+    if (!ids) {
+        const RgRange r = { 0 };
+        k_render_grid<V, RgRange><<<n_sel < cap ? n_sel : cap, RG_THREADS, smem, st>>>(lp, p->P, r, n_sel, rgb, lut, ts, highlight);
+        p->launches++;
+        return;
+    }
+    RgList l;
+    for (int32_t k0 = 0; k0 < n_sel; k0 += RG_IDS) {
+        const int m = n_sel - k0 < RG_IDS ? n_sel - k0 : RG_IDS;
+        memcpy(l.id, ids + k0, (size_t)m * sizeof(int32_t));
+        k_render_grid<V, RgList><<<m < cap ? m : cap, RG_THREADS, smem, st>>>(lp, p->P, l, m, rgb + (size_t)k0 * frame, lut, ts, highlight);
+        p->launches++;
+    }
 }
 
 extern "C" {
@@ -1158,6 +1288,40 @@ int bb_pool_render_rgb(bb_pool *p, const uint8_t *obs_dev, uint8_t *rgb_dev, int
     if (blocks > p->sm_count * 8) blocks = p->sm_count * 8;          // grid-stride over the envs: a multiple of the SM count
     k_render_rgb<<<blocks, RGB_THREADS, 0, (cudaStream_t)stream>>>(obs_dev, rgb_dev, p->d_rgb_lut, n_obs);
     p->launches++;
+    CU(cudaGetLastError());
+    return 0;
+}
+
+int bb_grid_tiles(int32_t tile_size, uint8_t *tiles_host)
+{
+    if (!tiles_host || tile_size < 1 || tile_size > bb_rgb::MAX_TILE_SIZE) return fail("bad arguments (tile_size must be 1..64)");
+    bb_rgb::render_grid_tiles(tile_size, tiles_host);
+    return 0;
+}
+
+int bb_pool_render_grid(bb_pool *p, const int32_t *env_ids_host, int32_t n_sel, int32_t tile_size, int32_t highlight,
+                        uint8_t *rgb_dev, void *stream)
+{
+    if (!p || n_sel < 0 || (n_sel > 0 && !rgb_dev)) return fail("bad arguments");
+    if (tile_size < 1 || tile_size > bb_rgb::MAX_TILE_SIZE) return fail("tile_size must be 1..64");
+    if (!env_ids_host && n_sel != p->n) return fail("env_ids_host = NULL renders every env: n_sel must equal n_envs");
+    if ((((uintptr_t)rgb_dev) & 15) != 0) return fail("rgb_dev must be 16-byte aligned");
+    if (env_ids_host)
+        for (int32_t k = 0; k < n_sel; k++)
+            if (env_ids_host[k] < 0 || env_ids_host[k] >= p->n) return fail("env id out of range [0, n_envs)");
+    CU(cudaSetDevice(p->device));
+    const uint8_t *lut = nullptr;
+    if (grid_table(p, tile_size, &lut)) return 1;
+    if (n_sel == 0) return 0;
+    // the widest store that divides the tile row (3 ts bytes): the lowest set bit of ts, at most 16
+    const int v = tile_size & -tile_size;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int hl = highlight ? 1 : 0;
+    if (v >= 16) launch_render_grid<16>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
+    else if (v == 8) launch_render_grid<8>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
+    else if (v == 4) launch_render_grid<4>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
+    else if (v == 2) launch_render_grid<2>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
+    else launch_render_grid<1>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
     CU(cudaGetLastError());
     return 0;
 }

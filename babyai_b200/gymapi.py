@@ -14,6 +14,8 @@ importable, entry points pointing here, so `gym.make(id)` returns these objects.
 import os
 from enum import IntEnum
 
+import numpy as np
+
 from .levels import LEVELS
 from .vecenv import EnvList, ManyEnvs, _spaces
 
@@ -41,7 +43,7 @@ class SingleEnv(object):
     """gym.Env-shaped view of a one-environment pool.  Like a gym env it does NOT reset itself: after `done`
     further steps repeat the terminal result until reset() (the pool's freeze mode, evaluate.py:72-78)."""
     Actions = Actions
-    metadata = {'render.modes': []}
+    metadata = {'render.modes': ['rgb_array']}
     reward_range = (0, 1)
 
     def __init__(self, level, seed=None, device=0, pool=None):
@@ -74,8 +76,34 @@ class SingleEnv(object):
         obs, reward, done, info = self._vec.step([int(action)])
         return obs[0], reward[0], done[0], info[0]
 
-    def render(self, mode='human'):
-        raise NotImplementedError('the pool renders nothing; observations are the 7x7x3 symbolic view')
+    def render(self, mode='human', close=False, highlight=True, tile_size=32):
+        """MiniGridEnv.render: 'rgb_array' returns the full grid as numpy uint8[H * tile_size, W * tile_size, 3] (drawn on the
+        device by bb_pool_render_grid); there is no window, so 'human' raises."""
+        if close:
+            return None
+        if mode != 'rgb_array':
+            raise NotImplementedError("render(%r): the pool has no window; use render('rgb_array')" % (mode,))
+        pool = self._vec.pool
+        if not hasattr(pool, 'render_grid'):
+            raise NotImplementedError('this pool cannot render')
+        return pool.render_grid(None, tile_size=tile_size, highlight=highlight)[0].cpu().numpy()
+
+    def _state(self):
+        return self._vec.pool.state(0)[1]
+
+    @property
+    def step_count(self):
+        """steps taken in the current episode (MiniGridEnv.step_count)"""
+        return self._state()['step_count']
+
+    @property
+    def agent_pos(self):
+        s = self._state()
+        return np.array((s['agent_x'], s['agent_y']))
+
+    @property
+    def agent_dir(self):
+        return self._state()['agent_dir']
 
     def close(self):
         self._vec.pool.close() if hasattr(self._vec.pool, 'close') else None

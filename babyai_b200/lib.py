@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(HERE, 'libbabyai_b200.so')
 # every entry point include/babyai_b200.h declares
 SYMBOLS = [
     'bb_pool_create', 'bb_pool_destroy', 'bb_pool_seed', 'bb_pool_set_mode', 'bb_pool_reset', 'bb_pool_step',
-    'bb_pool_step_timed', 'bb_pool_rollout', 'bb_pool_rollout_timed', 'bb_pool_step_host', 'bb_pool_reset_host', 'bb_pool_step_learner', 'bb_pool_mission_tokens', 'bb_pool_render_rgb', 'bb_rgb_tiles', 'bb_vocab_size',
+    'bb_pool_step_timed', 'bb_pool_rollout', 'bb_pool_rollout_timed', 'bb_pool_step_host', 'bb_pool_reset_host', 'bb_pool_step_learner', 'bb_pool_mission_tokens', 'bb_pool_render_rgb', 'bb_rgb_tiles', 'bb_pool_render_grid', 'bb_grid_tiles', 'bb_vocab_size',
     'bb_vocab_word', 'bb_pool_get_state', 'bb_pool_width', 'bb_pool_height', 'bb_pool_num_envs',
     'bb_pool_counters', 'bb_pool_launches', 'bb_last_error',
 ]
@@ -46,6 +46,8 @@ def load():
     L.bb_pool_step_learner.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     L.bb_pool_render_rgb.argtypes = [vp, vp, vp, i32, vp]
     L.bb_rgb_tiles.argtypes = [vp]
+    L.bb_pool_render_grid.argtypes = [vp, vp, i32, i32, i32, vp, vp]
+    L.bb_grid_tiles.argtypes = [i32, vp]
     L.bb_pool_mission_tokens.argtypes = [vp, C.POINTER(vp), C.POINTER(i32)]
     L.bb_vocab_size.restype = i32
     L.bb_vocab_word.restype = C.c_char_p

@@ -159,6 +159,33 @@ class BabyAIVecEnv(object):
         _lib.check(self.L.bb_pool_render_rgb(self.h, _ptr(obs), _ptr(out), obs.numel() // 147, self._stream()))
         return out
 
+    def render_grid(self, env_ids=None, tile_size=32, highlight=True, out=None):
+        """MiniGridEnv.render('rgb_array', highlight=highlight, tile_size=tile_size) of the selected envs' CURRENT states
+        (bb_pool_render_grid): uint8 [n_sel, H * tile_size, W * tile_size, 3] on the device.  env_ids: ids in [0, N) in any
+        order, repeats allowed (default: every env in order)."""
+        ts = int(tile_size)
+        if not 1 <= ts <= 64:
+            raise ValueError('tile_size must be in 1..64 (got %r)' % (tile_size,))
+        ids = None
+        n_sel = self.num_envs
+        if env_ids is not None:
+            if torch.is_tensor(env_ids):
+                env_ids = env_ids.cpu().numpy()
+            a = np.asarray(env_ids)
+            if a.ndim != 1 or (a.size and a.dtype.kind not in 'iu'):
+                raise ValueError('env_ids must be a 1-D sequence of integer env ids')
+            if a.size and (a.min() < 0 or a.max() >= self.num_envs):
+                raise ValueError('env ids must be in [0, %d)' % self.num_envs)
+            ids = np.ascontiguousarray(a, dtype=np.int32)
+            n_sel = ids.size
+        shape = (n_sel, self.height * ts, self.width * ts, 3)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.uint8, device=self.device)
+        _check(out, 'out', self.device, torch.uint8, shape)
+        _lib.check(self.L.bb_pool_render_grid(self.h, ids.ctypes.data_as(C.c_void_p) if ids is not None else None, n_sel, ts,
+                                              1 if highlight else 0, _ptr(out), self._stream()))
+        return out
+
     def step_timed(self, actions):
         """bb_pool_step with CUDA events around each kernel -> (ms k_step, ms k_gen)."""
         a, b = C.c_float(), C.c_float()

@@ -156,6 +156,22 @@ int bb_pool_render_rgb(bb_pool *pool, const uint8_t *obs_dev, uint8_t *rgb_dev, 
  * 256 for an unseen cell, 257 + cell byte for the agent's own cell.  For parity tests. */
 int bb_rgb_tiles(uint8_t *tiles_host);
 
+/* Replaces: MiniGridEnv.render('rgb_array', highlight=highlight, tile_size=tile_size) (gym_minigrid 1.0.x), what
+ * scripts/manual_control.py:14 draws and what video logging of agents needs: the full grid of each selected env's CURRENT
+ * state (after an auto-reset step: the first state of the new episode; in freeze mode: the terminal state).  Cell (x, y) is
+ * Grid.render_tile(cell, agent_dir if the agent stands there, highlight = the cell is visible in the agent's 7x7 view);
+ * the carried object and box contents are not drawn.  env_ids_host: n_sel ids in [0, n_envs), any order, repeats allowed;
+ * NULL = every env in order (n_sel must then be n_envs).  tile_size 1..64.  rgb_dev: uint8 [n_sel][H*ts][W*ts][3],
+ * 16-byte aligned.  Stream-ordered after the work already on `stream`, no synchronisation (the table of a tile size is
+ * rasterised on the host and uploaded the first time that size is rendered); arguments are checked before anything is
+ * launched. */
+int bb_pool_render_grid(bb_pool *pool, const int32_t *env_ids_host, int32_t n_sel, int32_t tile_size, int32_t highlight,
+                        uint8_t *rgb_dev, void *stream);
+/* The full-grid tile table of one tile size (host, no GPU): uint8 [2][5][43][ts][ts][3] indexed by highlight, agent (0 none,
+ * 1 + direction) and the cell index of a grid cell byte (0 empty, 1 + 6 k + color for k = wall / key / ball / box,
+ * 25 + 6 state + color for doors).  For parity tests. */
+int bb_grid_tiles(int32_t tile_size, uint8_t *tiles_host);
+
 /* Replaces: obs['mission'] + InstructionsPreprocessor (utils/format.py:59-75).
  * Device pointer to int16 [n_envs][max_len] token ids of the current missions
  * (0 = pad, ids index bb_vocab_word); rewritten whenever an env is reset. */
