@@ -534,6 +534,8 @@ struct bb_pool {
     long long rel;
     cudaStream_t stream;           // internal stream: host-buffer API, seeding, graph capture origin
     cudaStream_t gen_stream;       // level generation runs here, concurrently with the steps
+    cudaStream_t last_stream;      // the stream the previous call enqueued pool work on (order_after_last)
+    cudaEvent_t ev_last;           // recorded on last_stream when a call arrives on another stream
     cudaEvent_t ev_fork, ev_join;
     cudaEvent_t gen_ev[MAX_GEN_EVENTS];
     long long gens_enqueued;       // k index of the next k_gen in the current epoch
@@ -673,6 +675,18 @@ static int sched_join(bb_pool *p, cudaStream_t st)
     return 0;
 }
 
+// The pool orders its own state between streams; the caller orders its own buffers.  Every entry point that enqueues work on
+// the pool's state calls this first with the stream it enqueues on: when that differs from the stream of the previous such
+// call, `st` waits for everything enqueued on the previous stream so far.  On the same stream it enqueues nothing.
+static int order_after_last(bb_pool *p, cudaStream_t st)
+{
+    if (st == p->last_stream) return 0;
+    CU(cudaEventRecord(p->ev_last, p->last_stream));
+    CU(cudaStreamWaitEvent(st, p->ev_last, 0));
+    p->last_stream = st;
+    return 0;
+}
+
 // leaving rollout mode: the rings only hold >= D - T levels; make this a proper sync point again
 static int sched_leave_rollout(bb_pool *p, cudaStream_t st)
 {
@@ -684,19 +698,27 @@ static int sched_leave_rollout(bb_pool *p, cudaStream_t st)
     return 0;
 }
 
-// the device table of one tile size: rasterised on the host and uploaded on first use (through the pool's internal stream,
-// which only the pool's synchronous entry points use), kept until bb_pool_destroy
+// a tile table rasterised on the host, uploaded through the pool's internal stream (which only the pool's synchronous entry
+// points use) and kept until bb_pool_destroy.  The copy has landed when this returns, so a kernel on any stream may read the
+// table (a cudaMemcpy from pageable memory returns once the data is staged, and a non-blocking stream is not ordered after it).
+static int upload_table(bb_pool *p, const std::vector<uint8_t> &h, uint8_t **out)
+{
+    void *d = nullptr;
+    CU(cudaMalloc(&d, h.size()));
+    p->allocs.push_back(d);
+    CU(cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, p->stream));
+    CU(cudaStreamSynchronize(p->stream));
+    *out = (uint8_t *)d;
+    return 0;
+}
+
+// the device table of one tile size, rendered on first use
 static int grid_table(bb_pool *p, int ts, const uint8_t **lut)
 {
     if (!p->d_grid_lut[ts]) {
         std::vector<uint8_t> h((size_t)bb_rgb::GRID_TILES * ts * ts * 3);
         bb_rgb::render_grid_tiles(ts, h.data());
-        void *d = nullptr;
-        CU(cudaMalloc(&d, h.size()));
-        p->allocs.push_back(d);
-        CU(cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, p->stream));
-        CU(cudaStreamSynchronize(p->stream));
-        p->d_grid_lut[ts] = (uint8_t *)d;
+        if (upload_table(p, h, &p->d_grid_lut[ts])) return 1;
     }
     *lut = p->d_grid_lut[ts];
     return 0;
@@ -861,6 +883,8 @@ int bb_pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, bb
     CUP(cudaFuncSetAttribute(k_step8<8, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     CUP(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
     CUP(cudaEventCreateWithFlags(&p->ev_join, cudaEventDisableTiming));
+    CUP(cudaEventCreateWithFlags(&p->ev_last, cudaEventDisableTiming));
+    p->last_stream = p->stream;
     for (int i = 0; i < p->nev; i++) CUP(cudaEventCreateWithFlags(&p->gen_ev[i], cudaEventDisableTiming));
     CUP(cudaMallocHost((void **)&p->h_act, n));
     CUP(cudaMallocHost((void **)&p->h_obs, n * OBS_BYTES));
@@ -891,6 +915,7 @@ int bb_pool_destroy(bb_pool *p)
     for (int i = 0; i < p->nev; i++) if (p->gen_ev[i]) cudaEventDestroy(p->gen_ev[i]);
     if (p->ev_fork) cudaEventDestroy(p->ev_fork);
     if (p->ev_join) cudaEventDestroy(p->ev_join);
+    if (p->ev_last) cudaEventDestroy(p->ev_last);
     for (void *a : p->allocs) cudaFree(a);
     if (p->h_act) cudaFreeHost(p->h_act);
     if (p->h_obs) cudaFreeHost(p->h_obs);
@@ -910,6 +935,7 @@ int bb_pool_seed(bb_pool *p, const uint64_t *seeds_host)
     CU(cudaSetDevice(p->device));
     CU(cudaDeviceSynchronize());
     p->gen_outstanding = false; p->rel = 0; p->after_rollout = false; p->fused_T = 0;
+    p->last_stream = p->stream;                        // synchronous: nothing earlier is left to order after
     if (p->h_err) *p->h_err = 0;
     // stream-ordered copy: a synchronous cudaMemcpy from pageable memory may return before its last
     // chunk has landed, and p->stream (non-blocking) is not ordered after the legacy stream
@@ -928,6 +954,7 @@ int bb_pool_set_mode(bb_pool *p, int32_t mode)
     CU(cudaSetDevice(p->device));
     CU(cudaDeviceSynchronize());
     p->gen_outstanding = false; p->rel = 0; p->after_rollout = false;
+    p->last_stream = p->stream;
     p->mode = mode;
     if (mode == BB_MODE_AUTORESET) { launch_gen(p, p->stream); CU(cudaStreamSynchronize(p->stream)); }
     if (p->graph) { cudaGraphExecDestroy(p->graph); p->graph = nullptr; }
@@ -939,6 +966,7 @@ int bb_pool_reset(bb_pool *p, uint8_t *obs_dev, int8_t *dir_dev, void *stream)
     if (!p || !obs_dev) return fail("bad arguments");
     CU(cudaSetDevice(p->device));
     cudaStream_t st = (cudaStream_t)stream;
+    if (order_after_last(p, st)) return 1;
     if (sched_join(p, st)) return 1;
     p->after_rollout = false; p->rollouts = 0;
     launch_gen(p, st);                                 // make sure every ring holds a level
@@ -956,6 +984,7 @@ int bb_pool_step(bb_pool *p, const void *actions_dev, int32_t action_bytes, uint
     BB_CHECK_RINGS(p);
     CU(cudaSetDevice(p->device));
     cudaStream_t st = (cudaStream_t)stream;
+    if (order_after_last(p, st)) return 1;
     if (sched_leave_rollout(p, st)) return 1;
     if (sched_before_step(p, p->rel, st)) return 1;
     launch_step(p, actions_dev, action_bytes, obs_dev, reward_dev, done_dev, dir_dev, 0, st);
@@ -969,8 +998,11 @@ int bb_pool_step_timed(bb_pool *p, const void *actions_dev, int32_t action_bytes
                        uint8_t *done_dev, int8_t *dir_dev, float *ms_step, float *ms_gen)
 {
     if (!p || !actions_dev || !obs_dev || !reward_dev || !done_dev || !ms_step || !ms_gen) return fail("bad arguments");
+    if (action_bytes != 1 && action_bytes != 8) return fail("action_bytes must be 1 or 8");
+    BB_CHECK_RINGS(p);
     CU(cudaSetDevice(p->device));
     if (!p->ev[0]) for (int i = 0; i < 3; i++) CU(cudaEventCreate(&p->ev[i]));
+    if (order_after_last(p, p->stream)) return 1;
     if (sched_join(p, p->stream)) return 1;
     p->after_rollout = false;
     launch_gen(p, p->stream);                           // rings full before the timed pair
@@ -999,6 +1031,7 @@ int bb_pool_rollout(bb_pool *p, const int8_t *actions_dev, int32_t T, uint8_t *o
     BB_CHECK_RINGS(p);
     CU(cudaSetDevice(p->device));
     cudaStream_t user = (cudaStream_t)stream;
+    if (order_after_last(p, user)) return 1;          // before rollout_graph captures on the internal stream
     // Level supply of the persistent kernels.  In-stream refill passes (single-room levels without the fused generator warp):
     // one pass per `refill_every` launches, needs D >= (refill_every + 1) T.  Concurrent passes (multi-room levels: k_gen on
     // the side stream, beside the rollouts): a pass is forked at every R-th launch from a head snapshot taken before that
@@ -1190,6 +1223,7 @@ int bb_pool_step_host(bb_pool *p, const int8_t *actions_host, uint8_t *obs_host,
     }
     const bool direct = p->direct;
     const int zc = p->zc_level;
+    if (order_after_last(p, p->stream)) return 1;
     memcpy(p->h_act, actions_host, n);
     if (!zc) CU(cudaMemcpyAsync(p->d_act, p->h_act, n, cudaMemcpyHostToDevice, p->stream));
     if (sched_leave_rollout(p, p->stream)) return 1;
@@ -1234,6 +1268,7 @@ int bb_pool_step_learner(bb_pool *p, const int8_t *actions_host, uint8_t *obs_de
         else { cudaGetLastError(); p->lz_state = 2; }
     }
     const bool zc = p->lz_state == 1;
+    if (order_after_last(p, st)) return 1;
     memcpy(p->h_act, actions_host, n);
     if (!zc) CU(cudaMemcpyAsync(p->d_act, p->h_act, n, cudaMemcpyHostToDevice, st));
     if (sched_leave_rollout(p, st)) return 1;
@@ -1280,8 +1315,7 @@ int bb_pool_render_rgb(bb_pool *p, const uint8_t *obs_dev, uint8_t *rgb_dev, int
     if (!p->d_rgb_lut) {                                   // rasterise the tile table once (host), keep it on the device
         std::vector<uint8_t> lut((size_t)bb_rgb::N_TILES * bb_rgb::TILE_BYTES);
         bb_rgb::render_all_tiles(lut.data());
-        if (dalloc(p, &p->d_rgb_lut, lut.size())) return 1;
-        CU(cudaMemcpy(p->d_rgb_lut, lut.data(), lut.size(), cudaMemcpyHostToDevice));
+        if (upload_table(p, lut, &p->d_rgb_lut)) return 1;
     }
     if (n_obs == 0) return 0;
     int blocks = (n_obs + RGB_THREADS / 32 - 1) / (RGB_THREADS / 32);
@@ -1316,6 +1350,7 @@ int bb_pool_render_grid(bb_pool *p, const int32_t *env_ids_host, int32_t n_sel, 
     // the widest store that divides the tile row (3 ts bytes): the lowest set bit of ts, at most 16
     const int v = tile_size & -tile_size;
     cudaStream_t st = (cudaStream_t)stream;
+    if (order_after_last(p, st)) return 1;
     const int hl = highlight ? 1 : 0;
     if (v >= 16) launch_render_grid<16>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
     else if (v == 8) launch_render_grid<8>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);

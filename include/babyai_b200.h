@@ -12,6 +12,12 @@
  * pointers are CUDA device pointers on the pool's device (typically the
  * data_ptr() of PyTorch-owned tensors); `*_host` pointers are host memory.
  * `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
+ * Any call may use any stream, and the pool orders its own state between
+ * them: a call on a stream other than the previous call's waits for the pool
+ * work enqueued so far (the internal-stream calls -- *_host, *_timed -- too).
+ * The caller orders its own buffers, as in PyTorch: a buffer written on one
+ * stream and read by a call on another needs the caller's own event.  A
+ * stream handed to the pool must stay valid until the pool's next call.
  * Every function returns 0 on success, non-zero on error; bb_last_error()
  * returns a thread-local message.  A pool is used by one host thread at a
  * time, one outstanding step at a time (penv.py has the same contract).
