@@ -23,7 +23,7 @@ def __getattr__(name):
     if name in ('DemoRecorder', 'episodes_to_demos'):
         from . import demos
         return getattr(demos, name)
-    if name == 'gymapi':
+    if name in ('gymapi', 'evaluate'):
         import importlib
-        return importlib.import_module('.gymapi', __name__)
+        return importlib.import_module('.' + name, __name__)
     raise AttributeError(name)

@@ -8,6 +8,7 @@
 //                 smaller than 6x6): one lane per environment, the warp in lock-step through one attempt per round.
 //   k_gen         level generation for every other level: one warp per level (generate_level).
 //   k_seed        env.seed().
+//   k_seed_sel, k_gen_scan_sel, k_pub_sel, k_reset8  bb_pool_reset_envs: seed, refill and reset the envs of an id list only.
 //   k_render_rgb, k_render_grid  pictures: the partial view of an observation, and the full grid of an env's current state.
 // Levels depend only on the env's random stream, never on actions, so generating episodes k+1 .. k+D while episode k
 // is being played is equivalent to generating them at reset time: every env owns a ring of D pre-generated levels.
@@ -20,6 +21,7 @@
 #include <math.h>
 #include <new>
 #include <vector>
+#include <algorithm>
 #include <stdlib.h>
 
 #include "../../include/babyai_b200.h"
@@ -30,6 +32,7 @@
 #include "rollout_lane.cuh"
 #include "rollout_cta.cuh"
 #include "step8.cuh"
+#include "reset8.cuh"
 #include <type_traits>
 #include "rgb_tiles.h"
 #include "grid_render.cuh"
@@ -502,6 +505,70 @@ __global__ void k_seed(const PoolPtrs P, const uint64_t *seeds, const int n)
     P.attempts[env] = 0;
 }
 
+// ---- bb_pool_reset_envs: a new episode for the envs of an id list -----------------------------------------------------
+// The ids (and the seeds) travel by value in the launch parameters, in chunks, as k_render_grid's do: calls on different
+// streams share no device buffer.  Every kernel here touches the listed envs only, so a call costs O(n_sel), not O(n_envs).
+constexpr int RS_IDS = 4096, RS_SEEDS = 2048;
+struct RsList { int32_t id[RS_IDS]; };
+struct RsSeeds { int32_t id[RS_SEEDS]; uint64_t seed[RS_SEEDS]; };
+
+// k_seed for the listed envs
+__global__ void k_seed_sel(const PoolPtrs P, const __grid_constant__ RsSeeds sel, const int n_sel)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_sel) return;
+    const int env = sel.id[k];
+    RngRec r; r.seed = sel.seed[k]; r.draws = 0;
+    P.rng[env] = r;
+    P.locked_room[env] = 0xFF;
+    P.tail[env] = P.head[env];
+    P.tail_pub[env] = P.head[env];
+    P.attempts[env] = 0;
+}
+
+// k_gen_scan for the listed envs: the head snapshot of these envs only, onto the same four work lists (gen_count must be
+// cleared before the first chunk; the chunks of one call append)
+__global__ void k_gen_scan_sel(const PoolPtrs P, const __grid_constant__ RsList sel, const int n_sel, const int target)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    int b = -1, env = 0;
+    if (k < n_sel) {
+        env = sel.id[k];
+        const uint32_t hd = P.head[env];
+        P.head_snap[env] = hd;
+        const int missing = target - (int)(P.tail[env] - hd);
+        if (missing > 0) b = missing >= 4 ? 3 : missing - 1;
+    }
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        const uint32_t m = __ballot_sync(0xFFFFFFFFu, b == q);
+        if (m) {
+            int base = 0;
+            if (lane == 0) base = (int)atomicAdd(P.gen_count + q, (uint32_t)__popc(m));
+            base = __shfl_sync(0xFFFFFFFFu, base, 0);
+            if (b == q) P.gen_list[(size_t)q * P.n + base + __popc(m & ((1u << lane) - 1u))] = env;
+        }
+    }
+}
+
+// publishes tail_pub for the listed envs, after the generation pass that wrote their rings has completed
+__global__ void k_pub_sel(const PoolPtrs P, const __grid_constant__ RsList sel, const int n_sel)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n_sel) { const int env = sel.id[k]; P.tail_pub[env] = P.tail[env]; }
+}
+
+// the reset itself: reset8.cuh (also compiled, with the warp primitives emulated by threads, in tests/hostemu)
+template <bool UNTR>
+__global__ void __launch_bounds__(S8_THREADS)
+k_reset8(const LevelParams lp, const PoolPtrs P, const __grid_constant__ RsList sel, const int n_sel, uint8_t *__restrict__ obs,
+         int8_t *__restrict__ dirs)
+{
+    extern __shared__ __align__(16) uint8_t smem8[];
+    reset8_role<PoolPtrs, UNTR>(lp, P, sel.id, n_sel, obs, dirs, smem8, threadIdx.x & 31, threadIdx.x >> 5, blockIdx.x);
+}
+
 // ====================================== host side ======================================
 static thread_local char g_err[512] = "";
 static int fail(const char *fmt, const char *a = "")
@@ -581,20 +648,54 @@ static int make_params(const bb_level_spec *s, LevelParams *lp)
     return e ? fail("%s", e) : 0;
 }
 
+// the generator kernel of a pass, on the work lists a scan has built.  sel_envs > 0 (bb_pool_reset_envs): the lists hold at
+// most that many envs, and the grid is no wider than they need
+static void launch_gen_work(bb_pool *p, int target, cudaStream_t st, int max_rounds, int min_active, int min_keep, bool beside,
+                            int chain_cap, int sel_envs = 0)
+{
+    if (p->lp.small && !p->gen_generic) {
+        int blocks = p->gen_small_blocks;
+        if (sel_envs > 0 && (sel_envs + GS_THREADS - 1) / GS_THREADS < blocks) blocks = (sel_envs + GS_THREADS - 1) / GS_THREADS;
+        k_gen_small<<<blocks, GS_THREADS, 0, st>>>(p->lp, p->P, target, max_rounds, min_active, min_keep);
+    } else {
+        // blocks of a pass that runs BESIDE the rollout kernel (BB_GEN_BESIDE_BLOCKS_PER_SM, default = the full width): its
+        // resident blocks delay the next rollout launch's CTAs, but a
+        // narrower pass takes longer than the launches it overlaps and the join waits for it
+        int blocks = beside && p->gen_blocks_beside < p->gen_blocks ? p->gen_blocks_beside : p->gen_blocks;
+        if (sel_envs > 0 && (sel_envs + GEN_THREADS / 32 - 1) / (GEN_THREADS / 32) < blocks) blocks = (sel_envs + GEN_THREADS / 32 - 1) / (GEN_THREADS / 32);
+        if (p->lp.kind == KIND_IMPUNLOCK || p->lp.kind == KIND_UNLOCK || p->lp.kind == KIND_BONUS) k_gen<true><<<blocks, GEN_THREADS, 0, st>>>(p->lp, p->P, p->n, target, p->gen_lanes, chain_cap);
+        else k_gen<false><<<blocks, GEN_THREADS, 0, st>>>(p->lp, p->P, p->n, target, p->gen_lanes, chain_cap);
+    }
+}
+
 static void launch_gen_kernel(bb_pool *p, int target, cudaStream_t st, int max_rounds = 0, int min_active = 0, bool snap_heads = false, int min_keep = 0, bool beside = false, int chain_cap = 0)
 {
     cudaMemsetAsync(p->P.gen_count, 0, 8 * sizeof(uint32_t), st);      // list counters + work ticket
     k_gen_scan<<<(p->n + 255) / 256, 256, 0, st>>>(p->P, p->n, target, snap_heads ? 1 : 0);
     p->launches++;
-    if (p->lp.small && !p->gen_generic) {
-        k_gen_small<<<p->gen_small_blocks, GS_THREADS, 0, st>>>(p->lp, p->P, target, max_rounds, min_active, min_keep);
-    } else {
-        // blocks of a pass that runs BESIDE the rollout kernel (BB_GEN_BESIDE_BLOCKS_PER_SM, default = the full width): its
-        // resident blocks delay the next rollout launch's CTAs, but a
-        // narrower pass takes longer than the launches it overlaps and the join waits for it
-        const int blocks = beside && p->gen_blocks_beside < p->gen_blocks ? p->gen_blocks_beside : p->gen_blocks;
-        if (p->lp.kind == KIND_IMPUNLOCK || p->lp.kind == KIND_UNLOCK || p->lp.kind == KIND_BONUS) k_gen<true><<<blocks, GEN_THREADS, 0, st>>>(p->lp, p->P, p->n, target, p->gen_lanes, chain_cap);
-        else k_gen<false><<<blocks, GEN_THREADS, 0, st>>>(p->lp, p->P, p->n, target, p->gen_lanes, chain_cap);
+    launch_gen_work(p, target, st, max_rounds, min_active, min_keep, beside, chain_cap);
+}
+
+// A SELECTED generation pass (bb_pool_reset_envs): tops the rings of the listed envs up to `target` levels -- their head
+// snapshot (k_gen_scan_sel), the generator kernel launch_gen_kernel would pick, then their tail_pub.  Nothing else is read or
+// written, so it costs what the listed envs need, whatever the pool size.
+static void launch_gen_sel(bb_pool *p, const int32_t *ids, int32_t n_sel, int target, cudaStream_t st)
+{
+    cudaMemsetAsync(p->P.gen_count, 0, 8 * sizeof(uint32_t), st);
+    RsList l;
+    for (int32_t k0 = 0; k0 < n_sel; k0 += RS_IDS) {
+        const int m = n_sel - k0 < RS_IDS ? n_sel - k0 : RS_IDS;
+        memcpy(l.id, ids + k0, (size_t)m * sizeof(int32_t));
+        k_gen_scan_sel<<<(m + 255) / 256, 256, 0, st>>>(p->P, l, m, target);
+        p->launches++;
+    }
+    launch_gen_work(p, target, st, 0, 0, 0, false, 0, n_sel);
+    p->launches++;
+    for (int32_t k0 = 0; k0 < n_sel; k0 += RS_IDS) {
+        const int m = n_sel - k0 < RS_IDS ? n_sel - k0 : RS_IDS;
+        memcpy(l.id, ids + k0, (size_t)m * sizeof(int32_t));
+        k_pub_sel<<<(m + 255) / 256, 256, 0, st>>>(p->P, l, m);
+        p->launches++;
     }
 }
 
@@ -972,6 +1073,55 @@ int bb_pool_reset(bb_pool *p, uint8_t *obs_dev, int8_t *dir_dev, void *stream)
     launch_gen(p, st);                                 // make sure every ring holds a level
     launch_step(p, nullptr, 1, obs_dev, nullptr, nullptr, dir_dev, 1, st);
     if (p->mode == BB_MODE_AUTORESET) launch_gen(p, st);      // rings full again: a sync point
+    CU(cudaGetLastError());
+    return 0;
+}
+
+// A new episode for the listed envs only (DESIGN.md section 4.8).  After the join no generation pass writes a ring; the listed
+// envs are (re)seeded, a selected pass gives each listed ring its next level (freeze mode: 1, auto-reset: D), k_reset8 takes
+// it, and in auto-reset mode a second selected pass tops the listed rings back up to D -- so every ring is as deep as the
+// per-step schedule and the rollout paths assume (the unlisted ones are exactly as they were).
+int bb_pool_reset_envs(bb_pool *p, const int32_t *env_ids_host, const uint64_t *seeds_host, int32_t n_sel, uint8_t *obs_dev,
+                       int8_t *dir_dev, void *stream)
+{
+    if (!p || !obs_dev || n_sel < 0 || (n_sel > 0 && !env_ids_host)) return fail("bad arguments");
+    if (n_sel > p->n) return fail("more env ids than envs: an id is repeated");
+    for (int32_t k = 0; k < n_sel; k++)
+        if (env_ids_host[k] < 0 || env_ids_host[k] >= p->n) return fail("env id out of range [0, n_envs)");
+    {
+        std::vector<int32_t> s(env_ids_host, env_ids_host + n_sel);
+        std::sort(s.begin(), s.end());
+        if (std::adjacent_find(s.begin(), s.end()) != s.end()) return fail("env ids must not repeat");
+    }
+    BB_CHECK_RINGS(p);
+    CU(cudaSetDevice(p->device));
+    if (n_sel == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (order_after_last(p, st)) return 1;
+    if (sched_join(p, st)) return 1;                   // no generation pass is still writing rings on the side stream
+    if (seeds_host) {
+        RsSeeds s;
+        for (int32_t k0 = 0; k0 < n_sel; k0 += RS_SEEDS) {
+            const int m = n_sel - k0 < RS_SEEDS ? n_sel - k0 : RS_SEEDS;
+            memcpy(s.id, env_ids_host + k0, (size_t)m * sizeof(int32_t));
+            memcpy(s.seed, seeds_host + k0, (size_t)m * sizeof(uint64_t));
+            k_seed_sel<<<(m + 255) / 256, 256, 0, st>>>(p->P, s, m);
+            p->launches++;
+        }
+    }
+    const int target = p->mode == BB_MODE_AUTORESET ? p->D : 1;
+    launch_gen_sel(p, env_ids_host, n_sel, target, st);
+    const size_t sm8 = (size_t)S8_WARPS * 4 * (p->lp.cells_pad + S8_REC_FIXED) + (size_t)S8_WARPS * (S8_TILE_WORDS + 1) * 4;
+    RsList l;
+    for (int32_t k0 = 0; k0 < n_sel; k0 += RS_IDS) {
+        const int m = n_sel - k0 < RS_IDS ? n_sel - k0 : RS_IDS;
+        memcpy(l.id, env_ids_host + k0, (size_t)m * sizeof(int32_t));
+        const int blocks = (m + 4 * S8_WARPS - 1) / (4 * S8_WARPS);
+        if (p->lp.kind == KIND_UNLOCK) k_reset8<true><<<blocks, S8_THREADS, sm8, st>>>(p->lp, p->P, l, m, obs_dev, dir_dev);
+        else k_reset8<false><<<blocks, S8_THREADS, sm8, st>>>(p->lp, p->P, l, m, obs_dev, dir_dev);
+        p->launches++;
+    }
+    if (p->mode == BB_MODE_AUTORESET) launch_gen_sel(p, env_ids_host, n_sel, p->D, st);
     CU(cudaGetLastError());
     return 0;
 }

@@ -246,6 +246,22 @@ class DeviceManyEnvs(DeviceParallelEnv):
     def seed(self, seeds):
         self.pool.seed(list(seeds))
 
+    def reset_envs(self, env_ids, seeds, obs):
+        """env.seed(seeds[k]) + env.reset() for envs env_ids[k] (BabyAIVecEnv.reset_envs): returns `obs` -- the batch the last
+        step() returned -- with the rows of those envs replaced by their first observations and their new missions."""
+        img, dire = obs.image, obs.direction.clone()
+        if self.pixel:
+            raw = self._new_image()
+            self.pool.reset_envs(env_ids, seeds, obs=raw, direction=dire)
+            idx = torch.as_tensor(np.asarray(env_ids, dtype=np.int64), device=self.pool.device)
+            img = img.clone()
+            img[idx] = self.pool.render_rgb(raw[idx].contiguous())
+        else:
+            img = img.clone()
+            self.pool.reset_envs(env_ids, seeds, obs=img, direction=dire)
+        self._tokens = self.pool.mission_tokens.clone()
+        return ObsBatch(img, self._tokens, dire)
+
     def step(self, actions):
         obs, rew, done, info = super().step(actions)
         # evaluate.py:78 zips per-env result tuples; ModelAgent.analyze_feedback (utils/agent.py:76-82) tells a tuple of

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(HERE, 'libbabyai_b200.so')
 
 # every entry point include/babyai_b200.h declares
 SYMBOLS = [
-    'bb_pool_create', 'bb_pool_destroy', 'bb_pool_seed', 'bb_pool_set_mode', 'bb_pool_reset', 'bb_pool_step',
+    'bb_pool_create', 'bb_pool_destroy', 'bb_pool_seed', 'bb_pool_set_mode', 'bb_pool_reset', 'bb_pool_reset_envs', 'bb_pool_step',
     'bb_pool_step_timed', 'bb_pool_rollout', 'bb_pool_rollout_timed', 'bb_pool_step_host', 'bb_pool_reset_host', 'bb_pool_step_learner', 'bb_pool_mission_tokens', 'bb_pool_render_rgb', 'bb_rgb_tiles', 'bb_pool_render_grid', 'bb_grid_tiles', 'bb_vocab_size',
     'bb_vocab_word', 'bb_pool_get_state', 'bb_pool_width', 'bb_pool_height', 'bb_pool_num_envs',
     'bb_pool_counters', 'bb_pool_launches', 'bb_last_error',
@@ -37,6 +37,7 @@ def load():
     L.bb_pool_seed.argtypes = [vp, vp]
     L.bb_pool_set_mode.argtypes = [vp, i32]
     L.bb_pool_reset.argtypes = [vp, vp, vp, vp]
+    L.bb_pool_reset_envs.argtypes = [vp, vp, vp, i32, vp, vp, vp]
     L.bb_pool_step.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
     L.bb_pool_step_timed.argtypes = [vp, vp, i32, vp, vp, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     L.bb_pool_rollout.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]

@@ -114,6 +114,42 @@ class BabyAIVecEnv(object):
         _lib.check(self.L.bb_pool_reset(self.h, _ptr(obs), _ptr(direction), self._stream()))
         return obs
 
+    def _env_ids(self, env_ids):
+        """a 1-D sequence (list, numpy array or tensor) of env ids in [0, N) -> contiguous int32 numpy array"""
+        if torch.is_tensor(env_ids):
+            env_ids = env_ids.cpu().numpy()
+        a = np.asarray(env_ids)
+        if a.ndim != 1 or (a.size and a.dtype.kind not in 'iu'):
+            raise ValueError('env_ids must be a 1-D sequence of integer env ids')
+        if a.size and (a.min() < 0 or a.max() >= self.num_envs):
+            raise ValueError('env ids must be in [0, %d)' % self.num_envs)
+        return np.ascontiguousarray(a, dtype=np.int32)
+
+    def reset_envs(self, env_ids, seeds=None, obs=None, direction=None):
+        """A new episode for the listed envs only (bb_pool_reset_envs): env.seed(seeds[k]) if seeds are given, then
+        env.reset(), for env env_ids[k].  Without seeds an env takes the next level of its own stream.  Only the listed rows
+        of obs [N, 7, 7, 3] and direction [N] (default: the pool's own buffers) are written, and only their missions change;
+        in freeze mode the listed envs step again.  Ids must not repeat.  Returns obs."""
+        ids = self._env_ids(env_ids)
+        if np.unique(ids).size != ids.size:
+            raise ValueError('env ids must not repeat')
+        s = None
+        if seeds is not None:
+            if torch.is_tensor(seeds):
+                seeds = seeds.cpu().numpy()
+            s = np.ascontiguousarray(np.asarray(seeds, dtype=np.uint64))
+            if s.shape != ids.shape:
+                raise ValueError('seeds must have one value per env id (%d), got shape %s' % (ids.size, s.shape))
+        obs = self.obs if obs is None else obs
+        direction = self.direction if direction is None else direction
+        n = self.num_envs
+        _check(obs, 'obs', self.device, torch.uint8, (n, 7, 7, 3))
+        _check(direction, 'direction', self.device, torch.int8, (n,))
+        _lib.check(self.L.bb_pool_reset_envs(self.h, ids.ctypes.data_as(C.c_void_p),
+                                             s.ctypes.data_as(C.c_void_p) if s is not None else None, ids.size,
+                                             _ptr(obs), _ptr(direction), self._stream()))
+        return obs
+
     def step(self, actions, obs=None, reward=None, done=None, direction=None):
         """actions: CUDA tensor of N int8/uint8 or int64 values."""
         n = self.num_envs
@@ -169,14 +205,7 @@ class BabyAIVecEnv(object):
         ids = None
         n_sel = self.num_envs
         if env_ids is not None:
-            if torch.is_tensor(env_ids):
-                env_ids = env_ids.cpu().numpy()
-            a = np.asarray(env_ids)
-            if a.ndim != 1 or (a.size and a.dtype.kind not in 'iu'):
-                raise ValueError('env_ids must be a 1-D sequence of integer env ids')
-            if a.size and (a.min() < 0 or a.max() >= self.num_envs):
-                raise ValueError('env ids must be in [0, %d)' % self.num_envs)
-            ids = np.ascontiguousarray(a, dtype=np.int32)
+            ids = self._env_ids(env_ids)
             n_sel = ids.size
         shape = (n_sel, self.height * ts, self.width * ts, 3)
         if out is None:

@@ -104,6 +104,19 @@ int bb_pool_set_mode(bb_pool *pool, int32_t mode);
  * dir_dev: int8[n_envs] or NULL. */
 int bb_pool_reset(bb_pool *pool, uint8_t *obs_dev, int8_t *dir_dev, void *stream);
 
+/* Replaces: env.seed(seeds_host[k]) (if seeds_host != NULL) then env.reset() for the envs env_ids_host[0..n_sel) only
+ * (RoomGridLevel.reset, levelgen.py:35-47; make_agent_demos.py:93, evaluate.py:64-70 per env).  Each listed env starts a
+ * new episode: with seeds, the first level of seed seeds_host[k] (its state is then that of a pool that bb_pool_seed gave
+ * that seed, followed by bb_pool_reset: generation draws and attempts included); without, the next level of the env's own
+ * stream (what its next auto-reset would have taken).  In freeze mode the env steps again from the next call.  Envs not
+ * listed keep their state, level rings and streams.  obs_dev: uint8[n_envs][147], dir_dev: int8[n_envs] or NULL: only the
+ * rows of the listed envs are written; their mission tokens are rewritten.  Counters are unchanged (a reset ends no counted
+ * episode).  Ids must lie in [0, n_envs) without repeats; arguments are checked before anything is enqueued, and n_sel = 0
+ * enqueues nothing.  Asynchronous and stream-ordered on `stream`; the host arrays are consumed before the call returns.
+ * Device work scales with n_sel; in auto-reset mode a reseeded env's ring is refilled serially (D levels per env). */
+int bb_pool_reset_envs(bb_pool *pool, const int32_t *env_ids_host, const uint64_t *seeds_host, int32_t n_sel,
+                       uint8_t *obs_dev, int8_t *dir_dev, void *stream);
+
 /* Replaces: ParallelEnv.step (penv.py:45-52) / ManyEnvs.step (evaluate.py:72-78)
  * -> RoomGridLevel.step (levelgen.py:49-66) -> MiniGridEnv.step/gen_obs.
  * actions_dev: n_envs actions, action_bytes = 1 (int8/uint8) or 8 (int64, what
