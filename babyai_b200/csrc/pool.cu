@@ -10,6 +10,7 @@
 //   k_seed        env.seed().
 //   k_seed_sel, k_gen_scan_sel, k_pub_sel, k_reset8  bb_pool_reset_envs: seed, refill and reset the envs of an id list only.
 //   k_save_envs, k_load_envs, k_observe8  bb_pool_save_envs / bb_pool_load_envs: env records out of and into the pool (env_record.cuh).
+//   k_step8_sel   bb_pool_step_envs: one step of the envs of an id list, eight lanes per environment (step8_sel.cuh).
 //   k_render_rgb, k_render_grid  pictures: the partial view of an observation, and the full grid of an env's current state.
 // Levels depend only on the env's random stream, never on actions, so generating episodes k+1 .. k+D while episode k
 // is being played is equivalent to generating them at reset time: every env owns a ring of D pre-generated levels.
@@ -34,6 +35,7 @@
 #include "rollout_cta.cuh"
 #include "step8.cuh"
 #include "reset8.cuh"
+#include "step8_sel.cuh"
 #include "env_record.cuh"
 #include <type_traits>
 #include "rgb_tiles.h"
@@ -581,6 +583,18 @@ k_observe8(const LevelParams lp, const PoolPtrs P, const __grid_constant__ RsLis
     observe8_role<PoolPtrs, UNTR>(lp, P, sel.id, n_sel, obs, dirs, smem8, threadIdx.x & 31, threadIdx.x >> 5, blockIdx.x);
 }
 
+// ---- bb_pool_step_envs: one step of the envs of an id list, action k for env ids[k] (step8_sel.cuh; also compiled, with the
+// warp primitives emulated by threads, in tests/hostemu).  k_step8's CTA shape and shared memory over the list instead of the pool
+template <int ACT_BYTES, bool UNTR>
+__global__ void __launch_bounds__(S8_THREADS)
+k_step8_sel(const LevelParams lp, const PoolPtrs P, const __grid_constant__ RsList sel, const int n_sel, const void *__restrict__ actions,
+            uint8_t *__restrict__ obs, float *__restrict__ reward, uint8_t *__restrict__ done, int8_t *__restrict__ dirs, const int mode)
+{
+    extern __shared__ __align__(16) uint8_t smem8[];
+    step8_sel_role<PoolPtrs, ACT_BYTES, UNTR>(lp, P, sel.id, n_sel, actions, obs, reward, done, dirs, mode, smem8,
+                                              threadIdx.x & 31, threadIdx.x >> 5, blockIdx.x);
+}
+
 // ---- bb_pool_save_envs / bb_pool_load_envs: env records (env_record.cuh) out of and into the pool --------------------------
 // Pure data movement.  The ring is slot-major ([depth][n]), so one env's record is up to 5 (1 + D) separate pieces; the work
 // is split over (level, env) PAIRS, one warp per pair at a time with 128-bit accesses, so that a single BossLevel env (513
@@ -901,9 +915,13 @@ static int check_env_ids(const bb_pool *p, const int32_t *ids, int32_t n_sel)
     if (n_sel > p->n) return fail("more env ids than envs: an id is repeated");
     for (int32_t k = 0; k < n_sel; k++)
         if (ids[k] < 0 || ids[k] >= p->n) return fail("env id out of range [0, n_envs)");
-    std::vector<int32_t> s(ids, ids + n_sel);
-    std::sort(s.begin(), s.end());
-    if (std::adjacent_find(s.begin(), s.end()) != s.end()) return fail("env ids must not repeat");
+    std::vector<uint64_t> seen(((size_t)p->n + 63) / 64, 0);      // linear: a host check must not cost more than the launch
+    for (int32_t k = 0; k < n_sel; k++) {
+        uint64_t &w = seen[(size_t)ids[k] >> 6];
+        const uint64_t bit = 1ull << (ids[k] & 63);
+        if (w & bit) return fail("env ids must not repeat");
+        w |= bit;
+    }
     return 0;
 }
 
@@ -1057,6 +1075,10 @@ int bb_pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, bb
     CUP(cudaFuncSetAttribute(k_rollout<1, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     CUP(cudaFuncSetAttribute(k_step8<1, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     CUP(cudaFuncSetAttribute(k_step8<8, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    CUP(cudaFuncSetAttribute(k_step8_sel<1, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    CUP(cudaFuncSetAttribute(k_step8_sel<8, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    CUP(cudaFuncSetAttribute(k_step8_sel<1, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    CUP(cudaFuncSetAttribute(k_step8_sel<8, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     CUP(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
     CUP(cudaEventCreateWithFlags(&p->ev_join, cudaEventDisableTiming));
     CUP(cudaEventCreateWithFlags(&p->ev_last, cudaEventDisableTiming));
@@ -1269,6 +1291,47 @@ int bb_pool_step(bb_pool *p, const void *actions_dev, int32_t action_bytes, uint
     if (sched_leave_rollout(p, st)) return 1;
     if (sched_before_step(p, p->rel, st)) return 1;
     launch_step(p, actions_dev, action_bytes, obs_dev, reward_dev, done_dev, dir_dev, 0, st);
+    if (sched_after_step(p, p->rel, st)) return 1;
+    p->rel++;
+    CU(cudaGetLastError());
+    return 0;
+}
+
+// One step of the listed envs only (DESIGN.md section 4.10).  It is one step of the per-step schedule: sched_before_step waits
+// for the generation pass that step `rel` needs, and sched_after_step forks the next one when it is due.  That schedule only
+// assumes that an env consumes at most one ring level per step -- true here, since a listed env ends at most one episode and
+// an unlisted env none -- so the pass that serves a bb_pool_step serves a selected step too, whatever mix of both a caller
+// issues.  The ids travel by value in the launch parameters, in chunks of RS_IDS (one launch each); the actions stay on the device.
+int bb_pool_step_envs(bb_pool *p, const int32_t *env_ids_host, int32_t n_sel, const void *actions_dev, int32_t action_bytes,
+                      uint8_t *obs_dev, float *reward_dev, uint8_t *done_dev, int8_t *dir_dev, void *stream)
+{
+    if (!p || n_sel < 0 || (n_sel > 0 && (!env_ids_host || !actions_dev)) || !obs_dev || !reward_dev || !done_dev) return fail("bad arguments");
+    if (action_bytes != 1 && action_bytes != 8) return fail("action_bytes must be 1 or 8");
+    if (check_env_ids(p, env_ids_host, n_sel)) return 1;
+    BB_CHECK_RINGS(p);
+    CU(cudaSetDevice(p->device));
+    if (n_sel == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (order_after_last(p, st)) return 1;
+    if (sched_leave_rollout(p, st)) return 1;
+    if (sched_before_step(p, p->rel, st)) return 1;
+    const size_t sm8 = (size_t)S8_WARPS * 4 * (p->lp.cells_pad + S8_REC_FIXED) + (size_t)S8_WARPS * (S8_TILE_WORDS + 1) * 4;
+    const bool untr = p->lp.kind == KIND_UNLOCK;
+    RsList l;
+    for (int32_t k0 = 0; k0 < n_sel; k0 += RS_IDS) {
+        const int m = n_sel - k0 < RS_IDS ? n_sel - k0 : RS_IDS;
+        memcpy(l.id, env_ids_host + k0, (size_t)m * sizeof(int32_t));
+        const int blocks = (m + 4 * S8_WARPS - 1) / (4 * S8_WARPS);
+        const void *a = static_cast<const int8_t *>(actions_dev) + (size_t)k0 * action_bytes;
+        if (action_bytes == 8) {
+            if (untr) k_step8_sel<8, true><<<blocks, S8_THREADS, sm8, st>>>(p->lp, p->P, l, m, a, obs_dev, reward_dev, done_dev, dir_dev, p->mode);
+            else k_step8_sel<8, false><<<blocks, S8_THREADS, sm8, st>>>(p->lp, p->P, l, m, a, obs_dev, reward_dev, done_dev, dir_dev, p->mode);
+        } else {
+            if (untr) k_step8_sel<1, true><<<blocks, S8_THREADS, sm8, st>>>(p->lp, p->P, l, m, a, obs_dev, reward_dev, done_dev, dir_dev, p->mode);
+            else k_step8_sel<1, false><<<blocks, S8_THREADS, sm8, st>>>(p->lp, p->P, l, m, a, obs_dev, reward_dev, done_dev, dir_dev, p->mode);
+        }
+        p->launches++;
+    }
     if (sched_after_step(p, p->rel, st)) return 1;
     p->rel++;
     CU(cudaGetLastError());

@@ -235,6 +235,31 @@ class BabyAIVecEnv(object):
                                        _ptr(direction), self._stream()))
         return obs, reward, done
 
+    def step_envs(self, env_ids, actions, obs=None, reward=None, done=None, direction=None):
+        """One step of the listed envs only (bb_pool_step_envs), every other env held still: env env_ids[k] takes action
+        actions[k] -- a contiguous CUDA tensor of len(env_ids) int8 / uint8 / int64 values, what a policy evaluated on
+        obs[env_ids] returns.  Only the listed rows of obs [N, 7, 7, 3], reward [N], done [N] and direction [N] (default:
+        the pool's own buffers) are written, so they stay the pool's current view.  Ids must not repeat.  Returns
+        (obs, reward, done)."""
+        ids = self._env_ids(env_ids)
+        seen = np.zeros(self.num_envs, bool)                   # linear (np.unique sorts: more host time than the launch)
+        seen[ids] = True
+        if np.count_nonzero(seen) != ids.size:
+            raise ValueError('env ids must not repeat')
+        if not (torch.is_tensor(actions) and actions.is_cuda and actions.device == self.device and actions.is_contiguous()
+                and actions.numel() == ids.size and actions.dtype in (torch.int8, torch.uint8, torch.int64)):
+            raise ValueError('actions must be a contiguous CUDA tensor of %d int8 / uint8 / int64 values on %s (one per env id)'
+                             % (ids.size, self.device))
+        obs = self.obs if obs is None else obs
+        reward = self.reward if reward is None else reward
+        done = self.done if done is None else done
+        direction = self.direction if direction is None else direction
+        self._check_step_outputs(obs, reward, done, direction, ())
+        _lib.check(self.L.bb_pool_step_envs(self.h, ids.ctypes.data_as(C.c_void_p), ids.size, _ptr(actions),
+                                            actions.element_size(), _ptr(obs), _ptr(reward), _ptr(done), _ptr(direction),
+                                            self._stream()))
+        return obs, reward, done
+
     def _check_step_outputs(self, obs, reward, done, direction, lead):
         n = self.num_envs
         _check(obs, 'obs', self.device, torch.uint8, lead + (n, 7, 7, 3))

@@ -150,6 +150,22 @@ int bb_pool_load_envs(bb_pool *pool, const int32_t *env_ids_host, const int32_t 
 int bb_pool_step(bb_pool *pool, const void *actions_dev, int32_t action_bytes,
                  uint8_t *obs_dev, float *reward_dev, uint8_t *done_dev, int8_t *dir_dev, void *stream);
 
+/* Replaces: ManyEnvs.step (babyai/evaluate.py:72-78), which steps only the envs that are not done -- here any id list: one
+ * step of the listed envs, every other env held still.  The result equals bb_pool_step restricted to the listed envs: env
+ * env_ids_host[k] applies action k of actions_dev (indexed by LIST POSITION, like seeds_host of bb_pool_reset_envs: what a
+ * policy evaluated on obs[ids] returns) and writes ROW env_ids_host[k] of obs_dev uint8 [n_envs][147], reward_dev float32
+ * [n_envs], done_dev uint8 [n_envs] and dir_dev int8 [n_envs] (may be NULL) -- only the listed rows.  action_bytes: 1
+ * (int8 / uint8) or 8 (int64).  In auto-reset mode a listed env whose episode ends takes the next level of its ring and
+ * returns the terminal reward and done with the new episode's first observation (its mission tokens change); in freeze mode
+ * a listed frozen env replays its last reward with done = 1, as in bb_pool_step.  Unlisted envs do not move: their state,
+ * stream, step count, output rows and mission tokens stay as they were (a generation pass that falls due may top their
+ * rings up with the next levels of their own streams, as during any call).  The counters change as bb_pool_step would change
+ * them for the listed envs.  Ids lie in [0, n_envs) without repeats; every argument is checked before anything is enqueued,
+ * and n_sel = 0 enqueues nothing and is not a step.  Stream-ordered on `stream` like bb_pool_step, no synchronisation; the
+ * host id array is consumed before the call returns.  Device work scales with n_sel: one launch per 4 096 ids. */
+int bb_pool_step_envs(bb_pool *pool, const int32_t *env_ids_host, int32_t n_sel, const void *actions_dev, int32_t action_bytes,
+                      uint8_t *obs_dev, float *reward_dev, uint8_t *done_dev, int8_t *dir_dev, void *stream);
+
 /* bb_pool_step on the pool's internal stream with CUDA events around each of its
  * two kernels (measurement hook for bench.py's roofline line; synchronises). */
 int bb_pool_step_timed(bb_pool *pool, const void *actions_dev, int32_t action_bytes,
