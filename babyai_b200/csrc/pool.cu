@@ -234,8 +234,8 @@ struct SmemRoomKindMem : SmemOnlyMem {           // env_logic.cuh mem_spec: sing
 template <int ACT_BYTES, bool UNTR = false, int ROOM_KINDS = 0>
 __global__ void __launch_bounds__(R_THREADS_FUSED, 7)
 k_rollout(const LevelParams lp, const PoolPtrs P, const void *__restrict__ actions_v, uint8_t *__restrict__ obs,
-          float *__restrict__ reward, uint8_t *__restrict__ done, int8_t *__restrict__ dirs, const int n, const int T,
-          const int mode, const int force_reset, const int gen_rounds, const int gen_min_active)
+          float *__restrict__ reward, uint8_t *__restrict__ done, int8_t *__restrict__ dirs, const int n, const int row_stride,
+          const int T, const int mode, const int force_reset, const int gen_rounds, const int gen_min_active)
 {
     extern __shared__ __align__(16) uint32_t smr[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -250,7 +250,7 @@ k_rollout(const LevelParams lp, const PoolPtrs P, const void *__restrict__ actio
     }
     // stepping warps: rollout_lane.cuh (also compiled, with the warp primitives emulated by threads, in tests/hostemu)
     rollout_lane_step_warp<PoolPtrs, typename std::conditional<ROOM_KINDS != 0, SmemRoomKindMem<ROOM_KINDS>, SmemOnlyMem>::type, ACT_BYTES, UNTR>(lp, P, actions_v, obs, reward, done, dirs, n, T, mode, force_reset, fused,
-                                                                   smr + warp * warp_words, lane, blockIdx.x * R_WARPS + warp, s_done);
+                                                                   smr + warp * warp_words, lane, blockIdx.x * R_WARPS + warp, s_done, row_stride);
 }
 
 // k_rollout_cta -- bb_pool_rollout on MULTI-ROOM levels: 32 envs per CTA, a lane-per-env step phase and a 4-lanes-per-env
@@ -258,10 +258,11 @@ k_rollout(const LevelParams lp, const PoolPtrs P, const void *__restrict__ actio
 template <bool UNTR>
 __global__ void __launch_bounds__(RC_THREADS, 7)
 k_rollout_cta(const LevelParams lp, const PoolPtrs P, const int8_t *__restrict__ actions, uint8_t *__restrict__ obs,
-              float *__restrict__ reward, uint8_t *__restrict__ done, int8_t *__restrict__ dirs, const int n, const int T, const int mode)
+              float *__restrict__ reward, uint8_t *__restrict__ done, int8_t *__restrict__ dirs, const int n, const int row_stride,
+              const int T, const int mode)
 {
     extern __shared__ __align__(16) uint32_t smc[];
-    rollout_cta_role<PoolPtrs, UNTR>(lp, P, actions, obs, reward, done, dirs, n, T, mode, smc, threadIdx.x, blockIdx.x);
+    rollout_cta_role<PoolPtrs, UNTR>(lp, P, actions, obs, reward, done, dirs, n, T, mode, smc, threadIdx.x, blockIdx.x, row_stride);
 }
 // Level generation, decoupled from the step: tops every environment's ring up to `target` levels.
 //
@@ -686,9 +687,20 @@ struct bb_pool {
     cudaEvent_t tev[4]; bool time_rollout, tev_kernel, tev_refill;
     const void *chk_obs; bool direct;            // bb_pool_step_host: caller buffers are page-locked       // bb_pool_rollout_timed
     int lz_state; int8_t *lz_act; float *lz_rew; uint8_t *lz_done;   // bb_pool_step_learner: 0 = not probed, 1 = mapped staging, 2 = copies
+    bb_level_spec spec;
+    int row_stride;                // rows between the steps of bb_pool_rollout's [T][.] buffers: n, or the N of the mixed pool this pool is a group of
+    // a MIXED pool (bb_pool_create_mixed) owns no envs itself: group g is the ordinary pool groups[g], whose envs are rows
+    // [gstart[g], gstart[g] + groups[g]->n) of every buffer; rollouts run each group on its own stream gstreams[g]
+    std::vector<bb_pool *> groups; std::vector<int32_t> gstart;
+    std::vector<cudaStream_t> gstreams; std::vector<cudaEvent_t> gjoin;
 };
 
-static int ring_dry(const bb_pool *p) { return p->h_err && *reinterpret_cast<volatile const int *>(p->h_err) != 0; }
+static bool is_mixed(const bb_pool *p) { return !p->groups.empty(); }
+static int ring_dry(const bb_pool *p)
+{
+    for (const bb_pool *c : p->groups) if (ring_dry(c)) return 1;
+    return p->h_err && *reinterpret_cast<volatile const int *>(p->h_err) != 0;
+}
 
 template <typename T>
 static int dalloc(bb_pool *p, T **out, size_t count)
@@ -782,8 +794,8 @@ static void launch_step(bb_pool *p, const void *actions, int action_bytes, uint8
     if (!cols) {
         const size_t smem = (size_t)R_WARPS * rl_warp_words(p->lp) * 4;
         const int blocks = (p->n + 32 * R_WARPS - 1) / (32 * R_WARPS);
-        if (action_bytes == 8) k_rollout<8><<<blocks, R_THREADS, smem, st>>>(p->lp, p->P, actions, obs, rew, done, dirs, p->n, 1, p->mode, force_reset, 0, 0);
-        else k_rollout<1><<<blocks, R_THREADS, smem, st>>>(p->lp, p->P, actions, obs, rew, done, dirs, p->n, 1, p->mode, force_reset, 0, 0);
+        if (action_bytes == 8) k_rollout<8><<<blocks, R_THREADS, smem, st>>>(p->lp, p->P, actions, obs, rew, done, dirs, p->n, p->n, 1, p->mode, force_reset, 0, 0);
+        else k_rollout<1><<<blocks, R_THREADS, smem, st>>>(p->lp, p->P, actions, obs, rew, done, dirs, p->n, p->n, 1, p->mode, force_reset, 0, 0);
         p->launches++;
         return;
     }
@@ -941,13 +953,106 @@ static void launch_records(bb_pool *p, Kernel kernel, const int32_t *ids, const 
     }
 }
 
+// the store width of k_render_grid: the widest that divides the tile row (3 ts bytes), i.e. the lowest set bit of ts, at most 16
+static void launch_render_grid_ts(bb_pool *p, const int32_t *ids, int32_t n_sel, int ts, int hl, uint8_t *rgb, cudaStream_t st,
+                                  const uint8_t *lut)
+{
+    const int v = ts & -ts;
+    if (v >= 16) launch_render_grid<16>(p, ids, n_sel, ts, hl, rgb, st, lut);
+    else if (v == 8) launch_render_grid<8>(p, ids, n_sel, ts, hl, rgb, st, lut);
+    else if (v == 4) launch_render_grid<4>(p, ids, n_sel, ts, hl, rgb, st, lut);
+    else if (v == 2) launch_render_grid<2>(p, ids, n_sel, ts, hl, rgb, st, lut);
+    else launch_render_grid<1>(p, ids, n_sel, ts, hl, rgb, st, lut);
+}
+
+// ---- mixed pools (bb_pool_create_mixed; DESIGN.md section 4.11) ----------------------------------------------------------
+// Every entry point dispatches to the groups at its top, after the checks that do not depend on the level.  A whole-pool call
+// calls each group with the caller's pointers offset by the group's first row; an id-list call makes one call per maximal run of
+// consecutive list positions whose envs lie in one group, with the ids translated to the group's rows.
+static int group_of(const bb_pool *p, int32_t env)
+{
+    return (int)(std::upper_bound(p->gstart.begin(), p->gstart.end(), env) - p->gstart.begin()) - 1;
+}
+
+// f(g, k0, m, local_ids): list positions [k0, k0 + m) are the run, local_ids their ids as rows of group g (ids are in range)
+template <class F>
+static int for_each_run(const bb_pool *p, const int32_t *ids, int32_t n_sel, F f)
+{
+    std::vector<int32_t> local((size_t)n_sel);
+    for (int32_t k0 = 0; k0 < n_sel;) {
+        const int g = group_of(p, ids[k0]);
+        const int32_t s = p->gstart[g], e = s + p->groups[g]->n;
+        int32_t k = k0;
+        for (; k < n_sel && ids[k] >= s && ids[k] < e; k++) local[k] = ids[k] - s;
+        if (f(g, k0, k - k0, local.data() + k0)) return 1;
+        k0 = k;
+    }
+    return 0;
+}
+
+static int mixed_excluded(const char *what)
+{
+    return fail("%s is not available on a mixed pool (include/babyai_b200.h says why)", what);
+}
+
+// the rollout: every group on its own stream, forked from and joined back into the caller's stream, so that the persistent
+// kernels of different groups share the GPU
+static int mixed_rollout(bb_pool *p, const int8_t *actions, int32_t T, uint8_t *obs, float *rew, uint8_t *done, int8_t *dirs,
+                         cudaStream_t user)
+{
+    CU(cudaEventRecord(p->ev_fork, user));
+    for (size_t g = 0; g < p->groups.size(); g++) {
+        const size_t s = (size_t)p->gstart[g];
+        CU(cudaStreamWaitEvent(p->gstreams[g], p->ev_fork, 0));
+        if (bb_pool_rollout(p->groups[g], actions + s, T, obs + s * OBS_BYTES, rew + s, done + s, dirs ? dirs + s : nullptr,
+                            p->gstreams[g])) return 1;
+        CU(cudaEventRecord(p->gjoin[g], p->gstreams[g]));
+    }
+    for (size_t g = 0; g < p->groups.size(); g++) CU(cudaStreamWaitEvent(user, p->gjoin[g], 0));
+    return 0;
+}
+
+// one step of every group on `st` from device actions into device outputs (rows offset by the group's start)
+static int mixed_step(bb_pool *p, const void *actions, int32_t action_bytes, uint8_t *obs, float *rew, uint8_t *done, int8_t *dirs,
+                      cudaStream_t st)
+{
+    for (size_t g = 0; g < p->groups.size(); g++) {
+        const size_t s = (size_t)p->gstart[g];
+        if (bb_pool_step(p->groups[g], static_cast<const int8_t *>(actions) + s * action_bytes, action_bytes, obs + s * OBS_BYTES,
+                         rew + s, done + s, dirs ? dirs + s : nullptr, st)) return 1;
+    }
+    return 0;
+}
+
+static int mixed_render_grid(bb_pool *p, const int32_t *ids, int32_t n_sel, int ts, int hl, uint8_t *rgb, cudaStream_t st)
+{
+    std::vector<int32_t> all;
+    if (!ids) { all.resize((size_t)n_sel); for (int32_t k = 0; k < n_sel; k++) all[k] = k; ids = all.data(); }
+    const LevelParams &l0 = p->groups[group_of(p, ids[0])]->lp;
+    for (int32_t k = 1; k < n_sel; k++) {
+        const LevelParams &l = p->groups[group_of(p, ids[k])]->lp;
+        if (l.W != l0.W || l.H != l0.H) return fail("the envs of one render_grid call must share one grid size (on a mixed pool: one call per size)");
+    }
+    const size_t frame = (size_t)l0.H * l0.W * ts * ts * 3;
+    return for_each_run(p, ids, n_sel, [&](int g, int32_t k0, int32_t m, const int32_t *loc) {
+        bb_pool *c = p->groups[g];
+        const uint8_t *lut = nullptr;
+        if (grid_table(c, ts, &lut) || order_after_last(c, st)) return 1;
+        launch_render_grid_ts(c, loc, m, ts, hl, rgb + (size_t)k0 * frame, st, lut);
+        return 0;
+    });
+}
+
 extern "C" {
 
 const char *bb_last_error(void) { return g_err; }
 
 // inside bb_pool_create: a failing CUDA call releases everything allocated so far
 #define CUP(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { fail("CUDA error: %s", cudaGetErrorString(_e)); bb_pool_destroy(p); return 1; } } while (0)
-int bb_pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, bb_pool **out)
+// max_tokens > 0: the token width of the missions (a mixed pool's widest, >= the level's own); tok != NULL: the mission tokens
+// live there (the pool's rows of a mixed pool's array) instead of in an array of the pool's own; row_stride: see bb_pool
+static int pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, int32_t max_tokens, int16_t *tok, int32_t row_stride,
+                       bb_pool **out)
 {
     if (!spec || !out || n_envs < 1) return fail("bad arguments");
     int ndev = 0;
@@ -957,6 +1062,8 @@ int bb_pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, bb
     bb_pool *p = new (std::nothrow) bb_pool();
     if (!p) return fail("out of memory");
     if (make_params(spec, &p->lp)) { delete p; return 1; }
+    if (max_tokens > 0) p->lp.max_tokens = max_tokens;
+    p->spec = *spec; p->row_stride = row_stride;
     p->n = n_envs; p->device = device; p->mode = BB_MODE_AUTORESET;
     p->num_warps = (n_envs + 3) / 4 + 4;          // counter slots: the 8-lanes-per-env kernel has the most warps
     {
@@ -1032,7 +1139,7 @@ int bb_pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, bb
     PoolPtrs &P = p->P;
     P.depth = p->D; P.n = n_envs;
     if (dalloc(p, &P.grid, n * lp.cells_pad) || dalloc(p, &P.hot, n) || dalloc(p, &P.obj, n) || dalloc(p, &P.ins, n) ||
-        dalloc(p, &P.tok, n * lp.max_tokens) || dalloc(p, &P.rgrid, D * n * lp.cells_pad) || dalloc(p, &P.rhot, D * n) ||
+        (tok ? (P.tok = tok, 0) : dalloc(p, &P.tok, n * lp.max_tokens)) || dalloc(p, &P.rgrid, D * n * lp.cells_pad) || dalloc(p, &P.rhot, D * n) ||
         dalloc(p, &P.robj, D * n) || dalloc(p, &P.rins, D * n) || dalloc(p, &P.rtok, D * n * lp.max_tokens) ||
         dalloc(p, &P.head, n) || dalloc(p, &P.tail, n) || dalloc(p, &P.head_snap, n) || dalloc(p, &P.tail_pub, n) ||
         dalloc(p, &P.rng, n) || dalloc(p, &P.locked_room, n) || dalloc(p, &P.attempts, n) || dalloc(p, &P.last_reward, n) ||
@@ -1100,6 +1207,65 @@ int bb_pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, bb
     return 0;
 }
 
+int bb_pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, bb_pool **out)
+{
+    return pool_create(spec, n_envs, device, 0, nullptr, n_envs, out);
+}
+
+// A mixed pool: the groups are ordinary pools whose mission tokens are rows of one [N][L] array (L: the widest group's
+// max_tokens; every generator and swap-in writes and zero-pads a mission up to lp.max_tokens) and whose rollouts step
+// through the caller's [T][N] buffers with row stride N.  Its own allocations: that array and the staging buffers of the
+// host-buffer calls, which run every group on the mixed pool's stream and synchronise once.
+int bb_pool_create_mixed(const bb_level_spec *specs, const int32_t *counts, int32_t n_groups, int32_t device, bb_pool **out)
+{
+    if (!specs || !counts || !out || n_groups < 1) return fail("bad arguments");
+    long long total = 0;
+    int32_t L = 0;
+    for (int32_t g = 0; g < n_groups; g++) {
+        if (counts[g] < 1) return fail("every group needs at least one env");
+        total += counts[g];
+        if (total > INT32_MAX) return fail("a pool holds at most INT32_MAX envs");
+        LevelParams lp;
+        if (make_params(specs + g, &lp)) return 1;
+        if (lp.max_tokens > L) L = lp.max_tokens;
+    }
+    if (n_groups == 1) return bb_pool_create(specs, counts[0], device, out);
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("no CUDA device available (the pool has no CPU fallback)");
+    if (device < 0 || device >= ndev) return fail("bad device index");
+    CU(cudaSetDevice(device));
+    bb_pool *p = new (std::nothrow) bb_pool();
+    if (!p) return fail("out of memory");
+    const size_t n = (size_t)total;
+    p->n = (int)total; p->device = device; p->mode = BB_MODE_AUTORESET; p->lp.max_tokens = L; p->row_stride = (int)total;
+    if (dalloc(p, &p->P.tok, n * L) || dalloc(p, &p->d_act, n) || dalloc(p, &p->d_obs, n * OBS_BYTES) || dalloc(p, &p->d_rew, n) ||
+        dalloc(p, &p->d_done, n) || dalloc(p, &p->d_dir, n)) {
+        bb_pool_destroy(p);
+        return 1;
+    }
+    CUP(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+    CUP(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
+    CUP(cudaMallocHost((void **)&p->h_act, n));
+    CUP(cudaMallocHost((void **)&p->h_obs, n * OBS_BYTES));
+    CUP(cudaMallocHost((void **)&p->h_rew, n * sizeof(float)));
+    CUP(cudaMallocHost((void **)&p->h_done, n));
+    CUP(cudaMallocHost((void **)&p->h_dir, n));
+    int32_t s = 0;
+    for (int32_t g = 0; g < n_groups; g++) {
+        bb_pool *c = nullptr;
+        if (pool_create(specs + g, counts[g], device, L, p->P.tok + (size_t)s * L, (int32_t)total, &c)) { bb_pool_destroy(p); return 1; }
+        p->groups.push_back(c); p->gstart.push_back(s);
+        cudaStream_t fs = nullptr; cudaEvent_t ev = nullptr;
+        CUP(cudaStreamCreateWithFlags(&fs, cudaStreamNonBlocking));
+        p->gstreams.push_back(fs);
+        CUP(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        p->gjoin.push_back(ev);
+        s += counts[g];
+    }
+    *out = p;
+    return 0;
+}
+
 #undef CUP
 
 int bb_pool_destroy(bb_pool *p)
@@ -1107,6 +1273,9 @@ int bb_pool_destroy(bb_pool *p)
     if (!p) return 0;
     cudaSetDevice(p->device);
     cudaDeviceSynchronize();
+    for (bb_pool *c : p->groups) bb_pool_destroy(c);
+    for (cudaStream_t s : p->gstreams) cudaStreamDestroy(s);
+    for (cudaEvent_t e : p->gjoin) cudaEventDestroy(e);
     if (p->graph) cudaGraphExecDestroy(p->graph);
     for (int i = 0; i < 3; i++) if (p->ev[i]) cudaEventDestroy(p->ev[i]);
     for (int i = 0; i < 4; i++) if (p->tev[i]) cudaEventDestroy(p->tev[i]);
@@ -1130,6 +1299,8 @@ int bb_pool_destroy(bb_pool *p)
 int bb_pool_seed(bb_pool *p, const uint64_t *seeds_host)
 {
     if (!p || !seeds_host) return fail("bad arguments");
+    for (size_t g = 0; g < p->groups.size(); g++) if (bb_pool_seed(p->groups[g], seeds_host + p->gstart[g])) return 1;
+    if (is_mixed(p)) return 0;
     CU(cudaSetDevice(p->device));
     CU(cudaDeviceSynchronize());
     p->gen_outstanding = false; p->rel = 0; p->after_rollout = false; p->fused_T = 0;
@@ -1149,6 +1320,8 @@ int bb_pool_seed(bb_pool *p, const uint64_t *seeds_host)
 int bb_pool_set_mode(bb_pool *p, int32_t mode)
 {
     if (!p || (mode != BB_MODE_AUTORESET && mode != BB_MODE_FREEZE)) return fail("bad arguments");
+    for (bb_pool *c : p->groups) if (bb_pool_set_mode(c, mode)) return 1;
+    if (is_mixed(p)) { p->mode = mode; return 0; }
     CU(cudaSetDevice(p->device));
     CU(cudaDeviceSynchronize());
     p->gen_outstanding = false; p->rel = 0; p->after_rollout = false;
@@ -1162,6 +1335,11 @@ int bb_pool_set_mode(bb_pool *p, int32_t mode)
 int bb_pool_reset(bb_pool *p, uint8_t *obs_dev, int8_t *dir_dev, void *stream)
 {
     if (!p || !obs_dev) return fail("bad arguments");
+    for (size_t g = 0; g < p->groups.size(); g++) {
+        const size_t s = (size_t)p->gstart[g];
+        if (bb_pool_reset(p->groups[g], obs_dev + s * OBS_BYTES, dir_dev ? dir_dev + s : nullptr, stream)) return 1;
+    }
+    if (is_mixed(p)) return 0;
     CU(cudaSetDevice(p->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (order_after_last(p, st)) return 1;
@@ -1186,6 +1364,12 @@ int bb_pool_reset_envs(bb_pool *p, const int32_t *env_ids_host, const uint64_t *
     BB_CHECK_RINGS(p);
     CU(cudaSetDevice(p->device));
     if (n_sel == 0) return 0;
+    if (is_mixed(p))
+        return for_each_run(p, env_ids_host, n_sel, [&](int g, int32_t k0, int32_t m, const int32_t *loc) {
+            const size_t s = (size_t)p->gstart[g];
+            return bb_pool_reset_envs(p->groups[g], loc, seeds_host ? seeds_host + k0 : nullptr, m, obs_dev + s * OBS_BYTES,
+                                      dir_dev ? dir_dev + s : nullptr, stream);
+        });
     cudaStream_t st = (cudaStream_t)stream;
     if (order_after_last(p, st)) return 1;
     if (sched_join(p, st)) return 1;                   // no generation pass is still writing rings on the side stream
@@ -1216,13 +1400,18 @@ int bb_pool_reset_envs(bb_pool *p, const int32_t *env_ids_host, const uint64_t *
     return 0;
 }
 
-int64_t bb_pool_env_record_bytes(const bb_pool *p) { return p ? rec_bytes(p->lp, p->D) : 0; }
+int64_t bb_pool_env_record_bytes(const bb_pool *p)
+{
+    if (p && is_mixed(p)) { mixed_excluded("bb_pool_env_record_bytes"); return 0; }
+    return p ? rec_bytes(p->lp, p->D) : 0;
+}
 
 // Records of the listed envs (DESIGN.md section 4.9).  It reads `tail` and the ring slots, so like bb_pool_reset_envs it
 // first joins every generation pass that may still be moving them on the side stream.
 int bb_pool_save_envs(bb_pool *p, const int32_t *env_ids_host, int32_t n_sel, uint8_t *records_dev, void *stream)
 {
     if (!p || n_sel < 0 || (n_sel > 0 && !records_dev)) return fail("bad arguments");
+    if (is_mixed(p)) return mixed_excluded("bb_pool_save_envs");
     if (!env_ids_host && n_sel > 0 && n_sel != p->n) return fail("env_ids_host = NULL saves every env: n_sel must equal n_envs");
     if ((((uintptr_t)records_dev) & 15) != 0) return fail("records_dev must be 16-byte aligned");
     if (env_ids_host)
@@ -1246,6 +1435,7 @@ int bb_pool_load_envs(bb_pool *p, const int32_t *env_ids_host, const int32_t *sl
                       int32_t n_records, uint8_t *obs_dev, int8_t *dir_dev, void *stream)
 {
     if (!p || n_sel < 0 || n_records < 0 || (n_sel > 0 && !records_dev)) return fail("bad arguments");
+    if (is_mixed(p)) return mixed_excluded("bb_pool_load_envs");
     if (!env_ids_host && n_sel > 0 && n_sel != p->n) return fail("env_ids_host = NULL loads every env: n_sel must equal n_envs");
     if ((((uintptr_t)records_dev) & 15) != 0) return fail("records_dev must be 16-byte aligned");
     if (env_ids_host && check_env_ids(p, env_ids_host, n_sel)) return 1;
@@ -1287,6 +1477,7 @@ int bb_pool_step(bb_pool *p, const void *actions_dev, int32_t action_bytes, uint
     BB_CHECK_RINGS(p);
     CU(cudaSetDevice(p->device));
     cudaStream_t st = (cudaStream_t)stream;
+    if (is_mixed(p)) return mixed_step(p, actions_dev, action_bytes, obs_dev, reward_dev, done_dev, dir_dev, st);
     if (order_after_last(p, st)) return 1;
     if (sched_leave_rollout(p, st)) return 1;
     if (sched_before_step(p, p->rel, st)) return 1;
@@ -1311,6 +1502,13 @@ int bb_pool_step_envs(bb_pool *p, const int32_t *env_ids_host, int32_t n_sel, co
     BB_CHECK_RINGS(p);
     CU(cudaSetDevice(p->device));
     if (n_sel == 0) return 0;
+    if (is_mixed(p))          // actions stay indexed by list position: a run's are the ones at its first position onwards
+        return for_each_run(p, env_ids_host, n_sel, [&](int g, int32_t k0, int32_t m, const int32_t *loc) {
+            const size_t s = (size_t)p->gstart[g];
+            return bb_pool_step_envs(p->groups[g], loc, m, static_cast<const int8_t *>(actions_dev) + (size_t)k0 * action_bytes,
+                                     action_bytes, obs_dev + s * OBS_BYTES, reward_dev + s, done_dev + s, dir_dev ? dir_dev + s : nullptr,
+                                     stream);
+        });
     cudaStream_t st = (cudaStream_t)stream;
     if (order_after_last(p, st)) return 1;
     if (sched_leave_rollout(p, st)) return 1;
@@ -1342,6 +1540,7 @@ int bb_pool_step_timed(bb_pool *p, const void *actions_dev, int32_t action_bytes
                        uint8_t *done_dev, int8_t *dir_dev, float *ms_step, float *ms_gen)
 {
     if (!p || !actions_dev || !obs_dev || !reward_dev || !done_dev || !ms_step || !ms_gen) return fail("bad arguments");
+    if (is_mixed(p)) return mixed_excluded("bb_pool_step_timed");
     if (action_bytes != 1 && action_bytes != 8) return fail("action_bytes must be 1 or 8");
     BB_CHECK_RINGS(p);
     CU(cudaSetDevice(p->device));
@@ -1375,6 +1574,7 @@ int bb_pool_rollout(bb_pool *p, const int8_t *actions_dev, int32_t T, uint8_t *o
     BB_CHECK_RINGS(p);
     CU(cudaSetDevice(p->device));
     cudaStream_t user = (cudaStream_t)stream;
+    if (is_mixed(p)) return mixed_rollout(p, actions_dev, T, obs_dev, reward_dev, done_dev, dir_dev, user);
     if (order_after_last(p, user)) return 1;          // before rollout_graph captures on the internal stream
     // Level supply of the persistent kernels.  In-stream refill passes (single-room levels without the fused generator warp):
     // one pass per `refill_every` launches, needs D >= (refill_every + 1) T.  Concurrent passes (multi-room levels: k_gen on
@@ -1444,14 +1644,14 @@ int bb_pool_rollout(bb_pool *p, const int8_t *actions_dev, int32_t T, uint8_t *o
     if (p->rollout_cta) {                  // multi-room levels: 32 envs per CTA, step phase + 4-lanes-per-env observation phase
         const int blocks_c = (p->n + RC_ENVS - 1) / RC_ENVS;
         const size_t smc = (size_t)rc2_cta_words(p->lp) * 4;
-        if (p->lp.kind == KIND_UNLOCK) k_rollout_cta<true><<<blocks_c, RC_THREADS, smc, user>>>(p->lp, p->P, actions_dev, obs_dev, reward_dev, done_dev, dir_dev, p->n, T, p->mode);
-        else k_rollout_cta<false><<<blocks_c, RC_THREADS, smc, user>>>(p->lp, p->P, actions_dev, obs_dev, reward_dev, done_dev, dir_dev, p->n, T, p->mode);
+        if (p->lp.kind == KIND_UNLOCK) k_rollout_cta<true><<<blocks_c, RC_THREADS, smc, user>>>(p->lp, p->P, actions_dev, obs_dev, reward_dev, done_dev, dir_dev, p->n, p->row_stride, T, p->mode);
+        else k_rollout_cta<false><<<blocks_c, RC_THREADS, smc, user>>>(p->lp, p->P, actions_dev, obs_dev, reward_dev, done_dev, dir_dev, p->n, p->row_stride, T, p->mode);
     }
     else {
         const int gr = fused ? (p->gen_budget > 0 ? p->gen_budget : 1 << 20) : 0, gm = fused ? p->gen_min_active : 0;
         const int threads = fused ? R_THREADS_FUSED : R_THREADS;
         const size_t sm = fused ? smem + RG_AREA_WORDS * 4 : smem;
-#define BB_LAUNCH_ROLLOUT(...) k_rollout<__VA_ARGS__><<<blocks, threads, sm, user>>>(p->lp, p->P, actions_dev, obs_dev, reward_dev, done_dev, dir_dev, p->n, T, p->mode, 0, gr, gm)
+#define BB_LAUNCH_ROLLOUT(...) k_rollout<__VA_ARGS__><<<blocks, threads, sm, user>>>(p->lp, p->P, actions_dev, obs_dev, reward_dev, done_dev, dir_dev, p->n, p->row_stride, T, p->mode, 0, gr, gm)
         if (p->lp.kind == KIND_UNLOCK) BB_LAUNCH_ROLLOUT(1, true);                         // (never fused: not a small level)
         else if (p->room_kinds == (1 << I_GOTO)) BB_LAUNCH_ROLLOUT(1, false, 1 << I_GOTO);
         else if (p->room_kinds == (1 << I_PICKUP)) BB_LAUNCH_ROLLOUT(1, false, 1 << I_PICKUP);
@@ -1479,6 +1679,7 @@ int bb_pool_rollout_timed(bb_pool *p, const int8_t *actions_dev, int32_t T, uint
                           uint8_t *done_dev, int8_t *dir_dev, float *ms_rollout_kernel, float *ms_refill)
 {
     if (!p || !ms_rollout_kernel || !ms_refill) return fail("bad arguments");
+    if (is_mixed(p)) return mixed_excluded("bb_pool_rollout_timed");
     *ms_rollout_kernel = 0; *ms_refill = 0;
     p->time_rollout = true; p->tev_kernel = false; p->tev_refill = false;
     const int rc = bb_pool_rollout(p, actions_dev, T, obs_dev, reward_dev, done_dev, dir_dev, p->stream);
@@ -1500,7 +1701,7 @@ static int rollout_graph(bb_pool *p, const int8_t *actions_dev, int32_t T, uint8
     if (!p->graph || memcmp(&key, &p->gkey, sizeof key) != 0) {
         if (p->graph) { cudaGraphExecDestroy(p->graph); p->graph = nullptr; }
         cudaGraph_t g;
-        const size_t n = (size_t)p->n;
+        const size_t n = (size_t)p->row_stride;                // rows between steps of the caller's [T][.] buffers
         const long long l0 = p->launches;
         const bool saved_out = p->gen_outstanding;
         // the generation branch forks from and joins back into the origin stream inside the capture
@@ -1544,6 +1745,23 @@ int bb_pool_step_host(bb_pool *p, const int8_t *actions_host, uint8_t *obs_host,
     if (!p || !actions_host || !obs_host || !reward_host || !done_host) return fail("bad arguments");
     CU(cudaSetDevice(p->device));
     const size_t n = (size_t)p->n;
+    if (is_mixed(p)) {            // every group enqueued through the staging buffers, one synchronisation
+        BB_CHECK_RINGS(p);
+        memcpy(p->h_act, actions_host, n);
+        CU(cudaMemcpyAsync(p->d_act, p->h_act, n, cudaMemcpyHostToDevice, p->stream));
+        if (mixed_step(p, p->d_act, 1, p->d_obs, p->d_rew, p->d_done, p->d_dir, p->stream)) return 1;
+        CU(cudaMemcpyAsync(p->h_obs, p->d_obs, n * OBS_BYTES, cudaMemcpyDeviceToHost, p->stream));
+        CU(cudaMemcpyAsync(p->h_rew, p->d_rew, n * sizeof(float), cudaMemcpyDeviceToHost, p->stream));
+        CU(cudaMemcpyAsync(p->h_done, p->d_done, n, cudaMemcpyDeviceToHost, p->stream));
+        CU(cudaMemcpyAsync(p->h_dir, p->d_dir, n, cudaMemcpyDeviceToHost, p->stream));
+        CU(cudaStreamSynchronize(p->stream));
+        BB_CHECK_RINGS(p);
+        memcpy(obs_host, p->h_obs, n * OBS_BYTES);
+        memcpy(reward_host, p->h_rew, n * sizeof(float));
+        memcpy(done_host, p->h_done, n);
+        if (dir_host) memcpy(dir_host, p->h_dir, n);
+        return 0;
+    }
     // page-locked caller buffers (cudaHostAlloc / cudaHostRegister / torch pin_memory) are the DMA targets
     // themselves; pageable ones go through the pool's pinned staging buffers + a host memcpy
     // the probe result is cached per (obs, reward, done, dir) pointer set; the observation buffer is re-probed on every call
@@ -1604,6 +1822,19 @@ int bb_pool_step_learner(bb_pool *p, const int8_t *actions_host, uint8_t *obs_de
     CU(cudaSetDevice(p->device));
     cudaStream_t st = (cudaStream_t)stream;
     const size_t n = (size_t)p->n;
+    if (is_mixed(p)) {            // every group enqueued through the staging buffers, one synchronisation
+        BB_CHECK_RINGS(p);
+        memcpy(p->h_act, actions_host, n);
+        CU(cudaMemcpyAsync(p->d_act, p->h_act, n, cudaMemcpyHostToDevice, st));
+        if (mixed_step(p, p->d_act, 1, obs_dev, p->d_rew, p->d_done, dir_dev, st)) return 1;
+        CU(cudaMemcpyAsync(p->h_rew, p->d_rew, n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(p->h_done, p->d_done, n, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        BB_CHECK_RINGS(p);
+        memcpy(reward_host, p->h_rew, n * sizeof(float));
+        memcpy(done_host, p->h_done, n);
+        return 0;
+    }
     if (p->lz_state == 0) {
         void *da = nullptr, *dr = nullptr, *dd = nullptr;
         const bool ok = p->zerocopy > 0 && cudaHostGetDevicePointer(&da, p->h_act, 0) == cudaSuccess &&
@@ -1654,6 +1885,7 @@ int bb_rgb_tiles(uint8_t *tiles_host)
 int bb_pool_render_rgb(bb_pool *p, const uint8_t *obs_dev, uint8_t *rgb_dev, int32_t n_obs, void *stream)
 {
     if (!p || !obs_dev || !rgb_dev || n_obs < 0) return fail("bad arguments");
+    if (is_mixed(p)) return bb_pool_render_rgb(p->groups[0], obs_dev, rgb_dev, n_obs, stream);       // a pure function of the observation
     if ((((uintptr_t)rgb_dev) & 15) != 0) return fail("rgb_dev must be 16-byte aligned");
     CU(cudaSetDevice(p->device));
     if (!p->d_rgb_lut) {                                   // rasterise the tile table once (host), keep it on the device
@@ -1688,19 +1920,18 @@ int bb_pool_render_grid(bb_pool *p, const int32_t *env_ids_host, int32_t n_sel, 
         for (int32_t k = 0; k < n_sel; k++)
             if (env_ids_host[k] < 0 || env_ids_host[k] >= p->n) return fail("env id out of range [0, n_envs)");
     CU(cudaSetDevice(p->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    const int hl = highlight ? 1 : 0;
+    if (is_mixed(p)) {
+        if (n_sel > 0 && mixed_render_grid(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st)) return 1;
+        CU(cudaGetLastError());
+        return 0;
+    }
     const uint8_t *lut = nullptr;
     if (grid_table(p, tile_size, &lut)) return 1;
     if (n_sel == 0) return 0;
-    // the widest store that divides the tile row (3 ts bytes): the lowest set bit of ts, at most 16
-    const int v = tile_size & -tile_size;
-    cudaStream_t st = (cudaStream_t)stream;
     if (order_after_last(p, st)) return 1;
-    const int hl = highlight ? 1 : 0;
-    if (v >= 16) launch_render_grid<16>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
-    else if (v == 8) launch_render_grid<8>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
-    else if (v == 4) launch_render_grid<4>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
-    else if (v == 2) launch_render_grid<2>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
-    else launch_render_grid<1>(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
+    launch_render_grid_ts(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
     CU(cudaGetLastError());
     return 0;
 }
@@ -1723,6 +1954,7 @@ const char *bb_vocab_word(int32_t id) { return (id >= 0 && id < W_COUNT) ? VOCAB
 int bb_pool_get_state(bb_pool *p, int32_t env, uint8_t *grid_host, int32_t *info)
 {
     if (!p || env < 0 || env >= p->n || !grid_host || !info) return fail("bad arguments");
+    if (is_mixed(p)) { const int g = group_of(p, env); return bb_pool_get_state(p->groups[g], env - p->gstart[g], grid_host, info); }
     CU(cudaSetDevice(p->device));
     CU(cudaDeviceSynchronize());
     EnvHot h; ObjTab ot; RngRec r; uint32_t att;
@@ -1747,14 +1979,59 @@ int bb_pool_get_state(bb_pool *p, int32_t env, uint8_t *grid_host, int32_t *info
     return 0;
 }
 
-int32_t bb_pool_width(const bb_pool *p) { return p ? p->lp.W : 0; }
-int32_t bb_pool_height(const bb_pool *p) { return p ? p->lp.H : 0; }
+int32_t bb_pool_width(const bb_pool *p)
+{
+    int32_t w = p ? p->lp.W : 0;
+    if (p) for (const bb_pool *c : p->groups) w = std::max(w, c->lp.W);
+    return w;
+}
+int32_t bb_pool_height(const bb_pool *p)
+{
+    int32_t h = p ? p->lp.H : 0;
+    if (p) for (const bb_pool *c : p->groups) h = std::max(h, c->lp.H);
+    return h;
+}
 int32_t bb_pool_num_envs(const bb_pool *p) { return p ? p->n : 0; }
-int64_t bb_pool_launches(const bb_pool *p) { return p ? p->launches : 0; }
+int64_t bb_pool_launches(const bb_pool *p)
+{
+    if (!p) return 0;
+    int64_t l = p->launches;
+    for (const bb_pool *c : p->groups) l += c->launches;
+    return l;
+}
+
+int32_t bb_pool_num_groups(const bb_pool *p) { return p ? (is_mixed(p) ? (int32_t)p->groups.size() : 1) : 0; }
+
+int bb_pool_group(const bb_pool *p, int32_t g, int32_t *start, int32_t *count, bb_level_spec *spec_out)
+{
+    if (!p || g < 0 || g >= bb_pool_num_groups(p)) return fail("bad arguments");
+    const bb_pool *c = is_mixed(p) ? p->groups[g] : p;
+    if (start) *start = is_mixed(p) ? p->gstart[g] : 0;
+    if (count) *count = c->n;
+    if (spec_out) *spec_out = c->spec;
+    return 0;
+}
+
+int bb_pool_env_dims(const bb_pool *p, int32_t env, int32_t *w, int32_t *h)
+{
+    if (!p || env < 0 || env >= p->n || !w || !h) return fail("bad arguments");
+    const bb_pool *c = is_mixed(p) ? p->groups[group_of(p, env)] : p;
+    *w = c->lp.W; *h = c->lp.H;
+    return 0;
+}
 
 int bb_pool_counters(bb_pool *p, int64_t *out4)
 {
     if (!p || !out4) return fail("bad arguments");
+    if (is_mixed(p)) {
+        for (int k = 0; k < 4; k++) out4[k] = 0;
+        for (bb_pool *c : p->groups) {
+            int64_t o[4];
+            if (bb_pool_counters(c, o)) return 1;
+            for (int k = 0; k < 4; k++) out4[k] += o[k];
+        }
+        return 0;
+    }
     CU(cudaSetDevice(p->device));
     CU(cudaDeviceSynchronize());
     std::vector<unsigned long long> c((size_t)p->num_warps * 4);

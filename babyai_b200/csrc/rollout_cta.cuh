@@ -144,8 +144,10 @@ struct DeferGMem : SmemGMem {
 
 template <class PP, bool UNTR>
 BB_DEV void rollout_cta_role(const LevelParams &lp, const PP &P, const int8_t *actions, uint8_t *obs, float *reward, uint8_t *done,
-                             int8_t *dirs, const int n, const int T, const int mode, uint32_t *smem, const int tid, const int cta)
+                             int8_t *dirs, const int n, const int T, const int mode, uint32_t *smem, const int tid, const int cta,
+                             const int row_stride = 0)
 {
+    const size_t rs = row_stride ? (size_t)row_stride : (size_t)n;     // rows between steps of the [T][.] buffers (rollout_lane.cuh)
     const int lane = tid & 31, warp = tid >> 5;
     const int gs = rc_grid_stride(lp);
     const int env0 = cta * RC_ENVS;
@@ -204,7 +206,7 @@ BB_DEV void rollout_cta_role(const LevelParams &lp, const PP &P, const int8_t *a
             bool begin = false;
             uint32_t pose = 0;
             const int a = a_next;
-            if (valid_a && t + 1 < T) a_next = BB_LD_S8(actions + (size_t)(t + 1) * n + env_a);
+            if (valid_a && t + 1 < T) a_next = BB_LD_S8(actions + (t + 1) * rs + env_a);
             if (valid_a) {
                 float rew = 0.0f; bool dn = false;
                 if (!(h.dirflags & 4)) {
@@ -218,7 +220,7 @@ BB_DEV void rollout_cta_role(const LevelParams &lp, const PP &P, const int8_t *a
                 } else { rew = last_rew; dn = true; }
                 if (begin && !(consumed < avail && avail <= (uint32_t)P.depth)) { begin = false; n_err++; *P.err_flag = 1; }   // ring dry
                 pose = (uint32_t)h.x | ((uint32_t)h.y << 8) | ((uint32_t)(h.dirflags & 3) << 16) | ((uint32_t)carry_cell_of<UNTR>(h, mem_a) << 24);
-                const size_t oi = (size_t)t * n + env_a;
+                const size_t oi = t * rs + env_a;
                 if (reward) reward[oi] = rew;
                 if (done) done[oi] = dn ? 1 : 0;
             }
@@ -263,7 +265,7 @@ BB_DEV void rollout_cta_role(const LevelParams &lp, const PP &P, const int8_t *a
         const int el = (tid >> 2) & (RC_ENVS - 1), q = tid & 3;
         const bool valid_b = el < nv;
         const uint8_t *g_b = reinterpret_cast<const uint8_t *>(sg + el * gs);
-        const bool bulk_ok = nv == RC_ENVS && (((uintptr_t)(obs + (size_t)env0 * OBS_BYTES)) & 15) == 0 && (((size_t)n * OBS_BYTES) & 15) == 0;
+        const bool bulk_ok = nv == RC_ENVS && (((uintptr_t)(obs + (size_t)env0 * OBS_BYTES)) & 15) == 0 && ((rs * OBS_BYTES) & 15) == 0;
         for (int t = 0; t < T; t++) {
             BB_BAR_SYNC(RC_BAR_X, RC_THREADS);                     // step t is committed
             if (*s_any) {
@@ -312,7 +314,7 @@ BB_DEV void rollout_cta_role(const LevelParams &lp, const PP &P, const int8_t *a
             const uint32_t mine = (q & 1) ? (p1 | (v16 << 16)) : (v16 | (p1 << 16));
             const uint32_t other = BB_SHFL_XOR(mine, 2);
             const uint32_t blo = (q & 2) ? other : mine, bhi = (q & 2) ? mine : other;
-            if (valid_b && q == 0 && dirs) dirs[(size_t)t * n + env0 + el] = (int8_t)dir;
+            if (valid_b && q == 0 && dirs) dirs[t * rs + env0 + el] = (int8_t)dir;
             // ---- B2(t): process_vis, encode, stage into tile t & 1 ----
             uint32_t *tile = tiles + (t & 1) * RC_TILE_WORDS;
             uint32_t tlo = blo, thi = bhi;
@@ -339,7 +341,7 @@ BB_DEV void rollout_cta_role(const LevelParams &lp, const PP &P, const int8_t *a
             } else stage_record_words<21, 6>(tile, oA, 7 * el + 6, nextA);
             BB_FENCE_ASYNC_SMEM();                                 // tile writes -> visible to the copy engine
             BB_BAR_SYNC(RC_BAR_OBS, RC_OBS_THREADS);               // the tile is complete
-            uint8_t *dst = obs + ((size_t)t * n + env0) * OBS_BYTES;
+            uint8_t *dst = obs + (t * rs + env0) * OBS_BYTES;
             if (bulk_ok) {
                 // the other tile is rewritten at step t + 1: its bulk copy (step t - 1) must have read it by then; every
                 // observer passes barrier X of step t + 1 only after this thread has

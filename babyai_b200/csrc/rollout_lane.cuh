@@ -52,8 +52,12 @@ BB_DEV void rl_store_tile_plain(const uint32_t *tile, uint8_t *dst, int lane, in
 template <class PP, class MemT, int ACT_BYTES, bool UNTR>
 BB_DEV void rollout_lane_step_warp(const LevelParams &lp, const PP &P, const void *actions_v, uint8_t *obs, float *reward, uint8_t *done,
                                    int8_t *dirs, const int n, const int T, const int mode, const int force_reset, const bool fused,
-                                   uint32_t *warp_smem, const int lane, const int warp_global, volatile int *s_done)
+                                   uint32_t *warp_smem, const int lane, const int warp_global, volatile int *s_done,
+                                   const int row_stride = 0)
 {
+    // rows between the steps of the [T][.] action and output buffers: n for a pool's own buffers (0), the mixed pool's env
+    // count for a group of a mixed pool (its rows are a column block of the caller's buffers)
+    const size_t rs = row_stride ? (size_t)row_stride : (size_t)n;
     const int8_t *actions = reinterpret_cast<const int8_t *>(actions_v);
     const int gs = (lp.cells_pad >> 2) | 1;
     const int env0 = warp_global * 32, env = env0 + lane;
@@ -93,7 +97,7 @@ BB_DEV void rollout_lane_step_warp(const LevelParams &lp, const PP &P, const voi
     }
     for (int t = 0; t < T; t++) {
         const int a = a_next;
-        if (ACT_BYTES == 1 && valid && t + 1 < T) a_next = BB_LD_S8(actions + (size_t)(t + 1) * n + env);
+        if (ACT_BYTES == 1 && valid && t + 1 < T) a_next = BB_LD_S8(actions + (t + 1) * rs + env);
         float rew = 0.0f; bool dn = false, begin = false;
         if (valid) {
             begin = force_reset != 0;
@@ -158,7 +162,7 @@ BB_DEV void rollout_lane_step_warp(const LevelParams &lp, const PP &P, const voi
                 BB_PREFETCH_L2(o.tok);
             }
             observe(lp, mem, h.x, h.y, h.dirflags & 3, carry_cell_of<UNTR>(h, mem), w);
-            const size_t oi = (size_t)t * n + env;
+            const size_t oi = t * rs + env;
             if (reward) reward[oi] = rew;
             if (done) done[oi] = dn ? 1 : 0;
             if (dirs) dirs[oi] = (int8_t)(h.dirflags & 3);
@@ -171,7 +175,7 @@ BB_DEV void rollout_lane_step_warp(const LevelParams &lp, const PP &P, const voi
             const uint32_t next_w0 = BB_SHFL_DOWN(w[0], 1);
             stage_obs_words(tile, w, lane, next_w0);
         }
-        uint8_t *dst = obs + ((size_t)t * n + env0) * OBS_BYTES;
+        uint8_t *dst = obs + (t * rs + env0) * OBS_BYTES;
         const bool bulk = nv == 32 && (((uintptr_t)dst) & 15) == 0;
         if (bulk) BB_FENCE_ASYNC_SMEM();                           // generic-proxy tile writes -> visible to the async proxy
         BB_SYNCWARP();

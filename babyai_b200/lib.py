@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(HERE, 'libbabyai_b200.so')
 
 # every entry point include/babyai_b200.h declares
 SYMBOLS = [
-    'bb_pool_create', 'bb_pool_destroy', 'bb_pool_seed', 'bb_pool_set_mode', 'bb_pool_reset', 'bb_pool_reset_envs', 'bb_pool_env_record_bytes',
+    'bb_pool_create', 'bb_pool_create_mixed', 'bb_pool_num_groups', 'bb_pool_group', 'bb_pool_env_dims', 'bb_pool_destroy', 'bb_pool_seed', 'bb_pool_set_mode', 'bb_pool_reset', 'bb_pool_reset_envs', 'bb_pool_env_record_bytes',
     'bb_pool_save_envs', 'bb_pool_load_envs', 'bb_pool_step', 'bb_pool_step_envs',
     'bb_pool_step_timed', 'bb_pool_rollout', 'bb_pool_rollout_timed', 'bb_pool_step_host', 'bb_pool_reset_host', 'bb_pool_step_learner', 'bb_pool_mission_tokens', 'bb_pool_render_rgb', 'bb_rgb_tiles', 'bb_pool_render_grid', 'bb_grid_tiles', 'bb_vocab_size',
     'bb_vocab_word', 'bb_pool_get_state', 'bb_pool_width', 'bb_pool_height', 'bb_pool_num_envs',
@@ -34,6 +34,11 @@ def load():
     L = C.CDLL(LIB_PATH)
     vp, i32, i64 = C.c_void_p, C.c_int32, C.c_int64
     L.bb_pool_create.argtypes = [C.POINTER(LevelSpec), i32, i32, C.POINTER(vp)]
+    L.bb_pool_create_mixed.argtypes = [C.POINTER(LevelSpec), C.POINTER(i32), i32, i32, C.POINTER(vp)]
+    L.bb_pool_num_groups.restype = i32
+    L.bb_pool_num_groups.argtypes = [vp]
+    L.bb_pool_group.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(LevelSpec)]
+    L.bb_pool_env_dims.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32)]
     L.bb_pool_destroy.argtypes = [vp]
     L.bb_pool_seed.argtypes = [vp, vp]
     L.bb_pool_set_mode.argtypes = [vp, i32]

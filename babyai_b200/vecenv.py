@@ -21,7 +21,7 @@ import numpy as np
 import torch
 
 from . import lib as _lib
-from .levels import VOCAB, detokenize, level_spec
+from .levels import VOCAB, LevelSpec, detokenize, level_spec
 
 MODE_AUTORESET, MODE_FREEZE = 0, 1
 
@@ -50,23 +50,67 @@ def _check(t, name, device, dtype, shape):
         raise ValueError('%s must be a contiguous %s tensor of shape %s (got %s %s)' % (name, dtypes[0], tuple(shape), t.dtype, tuple(t.shape)))
 
 
-class BabyAIVecEnv(object):
-    """N environments of one BabyAI level living in HBM of one GPU."""
+def level_groups(level):
+    """A level name -> None.  A dict {level_name: count} or a sequence of (level_name, count) pairs -> the list of
+    (level_name, count) groups of a mixed pool, in order (a level may appear in several groups)."""
+    if isinstance(level, str):
+        return None
+    items = list(level.items()) if isinstance(level, dict) else list(level)
+    groups = []
+    for item in items:
+        if not (isinstance(item, (tuple, list)) and len(item) == 2 and isinstance(item[0], str)):
+            raise ValueError('a mixed pool is given as (level_name, count) pairs, got %r' % (item,))
+        name, count = item
+        if isinstance(count, bool) or int(count) != count or count < 1:
+            raise ValueError('every group needs a whole number of envs >= 1, got %r for %s' % (count, name))
+        level_spec(name)                                   # unknown levels fail here, before anything is allocated
+        groups.append((name, int(count)))
+    if not groups:
+        raise ValueError('a mixed pool needs at least one (level_name, count) group')
+    if sum(c for _, c in groups) > 2 ** 31 - 1:
+        raise ValueError('a pool holds at most 2**31 - 1 envs')
+    return groups
 
-    def __init__(self, level, num_envs, seeds=None, device=0, mode=MODE_AUTORESET):
+
+class BabyAIVecEnv(object):
+    """N environments of one BabyAI level living in HBM of one GPU -- or, with `level` a sequence of (level_name, count)
+    pairs, a MIXED pool: group g holds envs [start, start + count) of its level (`groups`), each group stepped by its own
+    level's kernels, every buffer indexed by env row as for one level (bb_pool_create_mixed)."""
+
+    def __init__(self, level, num_envs=None, seeds=None, device=0, mode=MODE_AUTORESET):
         self.L = _lib.load()
         if not torch.cuda.is_available():
             raise RuntimeError('babyai_b200 needs a CUDA device; there is no CPU fallback')
         self.level = level
-        self.num_envs = int(num_envs)
+        pairs = level_groups(level)
+        if pairs is None:
+            pairs = [(level, int(num_envs))]
+        elif num_envs is not None and int(num_envs) != sum(c for _, c in pairs):
+            raise ValueError('num_envs (%d) is not the sum of the group sizes (%d)' % (num_envs, sum(c for _, c in pairs)))
+        self.num_envs = sum(c for _, c in pairs)
         self.device = torch.device('cuda', device)
-        self.spec = level_spec(level)
+        starts = np.cumsum([0] + [c for _, c in pairs])[:-1]
+        self.groups = [(name, int(s), c) for (name, c), s in zip(pairs, starts)]
+        self.mixed = len(self.groups) > 1
+        self._starts = np.asarray(starts, np.int64)
         h = C.c_void_p()
         torch.cuda.set_device(self.device)
-        _lib.check(self.L.bb_pool_create(C.byref(self.spec), self.num_envs, device, C.byref(h)))
+        if self.mixed:
+            self.spec = None
+            specs = (LevelSpec * len(pairs))(*[level_spec(name) for name, _ in pairs])
+            counts = (C.c_int32 * len(pairs))(*[c for _, c in pairs])
+            _lib.check(self.L.bb_pool_create_mixed(specs, counts, len(pairs), device, C.byref(h)))
+        else:
+            self.spec = level_spec(pairs[0][0])
+            _lib.check(self.L.bb_pool_create(C.byref(self.spec), self.num_envs, device, C.byref(h)))
         self.h = h
-        self.width = self.L.bb_pool_width(h)
+        self.width = self.L.bb_pool_width(h)              # a mixed pool: the largest grid of its groups
         self.height = self.L.bb_pool_height(h)
+        self._dims = []                                    # (width, height) of each group
+        for _, s, _ in self.groups:
+            w, hh = C.c_int32(), C.c_int32()
+            _lib.check(self.L.bb_pool_env_dims(h, s, C.byref(w), C.byref(hh)))
+            self._dims.append((w.value, hh.value))
         n = self.num_envs
         self.obs = torch.zeros((n, 7, 7, 3), dtype=torch.uint8, device=self.device)
         self.reward = torch.zeros(n, dtype=torch.float32, device=self.device)
@@ -81,6 +125,21 @@ class BabyAIVecEnv(object):
             self.set_mode(mode)
         if seeds is not None:
             self.seed(seeds)
+
+    def group_of(self, env_ids):
+        """index into `groups` of each env id"""
+        return np.searchsorted(self._starts, np.asarray(env_ids), side='right') - 1
+
+    def level_of(self, env):
+        """the level name of env `env`"""
+        if not 0 <= int(env) < self.num_envs:
+            raise IndexError(env)
+        return self.groups[int(self.group_of(int(env)))][0]
+
+    def _single_level(self, what):
+        if self.mixed:
+            raise RuntimeError('%s is not available on a mixed pool: an env record does not name its level, so a record of '
+                               'one group could load silently into an env of another level' % what)
 
     def close(self):
         if getattr(self, 'h', None) is not None and self.h:
@@ -158,6 +217,7 @@ class BabyAIVecEnv(object):
     @property
     def record_bytes(self):
         """bytes of one env record: the row length of the tensors save_envs returns and load_envs takes"""
+        self._single_level('record_bytes')
         return int(self.L.bb_pool_env_record_bytes(self.h))
 
     def _check_records(self, records, name, rows=None):
@@ -172,6 +232,7 @@ class BabyAIVecEnv(object):
         (`out`, or a new tensor).  A record holds everything the env's future depends on, the levels its generator has
         already produced included, so load_envs of it continues exactly as the env would have.  The pool is unchanged; ids
         may repeat.  `torch.save(records.cpu(), path)` of the result is a checkpoint of the env side of a run."""
+        self._single_level('save_envs')
         ids = None if ids is None else self._env_ids(ids)
         n_sel = self.num_envs if ids is None else ids.size
         if out is None:
@@ -186,6 +247,7 @@ class BabyAIVecEnv(object):
         returned on a pool of the same level and ring depth.  Slots may repeat (one record into many envs), ids may not.
         Only the listed rows of obs / direction (default: the pool's own buffers) are written -- the observations of the
         loaded states -- and only the listed envs' missions change; unlisted envs are untouched.  Returns (obs, direction)."""
+        self._single_level('load_envs')
         self._check_records(records, 'records')
         ids = None if ids is None else self._env_ids(ids)
         if ids is not None and np.unique(ids).size != ids.size:
@@ -211,6 +273,7 @@ class BabyAIVecEnv(object):
         """Env dst_ids[k] becomes a copy of env src_ids[k] as it is now (copy.deepcopy of a reference env): sources may
         repeat, destinations may not, and a destination may also be a source (every source is saved before any env is
         loaded).  Returns (obs, direction) as load_envs does."""
+        self._single_level('copy_envs')
         src, dst = self._env_ids(src_ids), self._env_ids(dst_ids)
         if src.shape != dst.shape:
             raise ValueError('src_ids and dst_ids must have the same length')
@@ -292,7 +355,8 @@ class BabyAIVecEnv(object):
     def render_grid(self, env_ids=None, tile_size=32, highlight=True, out=None):
         """MiniGridEnv.render('rgb_array', highlight=highlight, tile_size=tile_size) of the selected envs' CURRENT states
         (bb_pool_render_grid): uint8 [n_sel, H * tile_size, W * tile_size, 3] on the device.  env_ids: ids in [0, N) in any
-        order, repeats allowed (default: every env in order)."""
+        order, repeats allowed (default: every env in order).  On a mixed pool the selected envs must share one grid size
+        (H, W: the level's own), e.g. one group per call."""
         ts = int(tile_size)
         if not 1 <= ts <= 64:
             raise ValueError('tile_size must be in 1..64 (got %r)' % (tile_size,))
@@ -301,7 +365,14 @@ class BabyAIVecEnv(object):
         if env_ids is not None:
             ids = self._env_ids(env_ids)
             n_sel = ids.size
-        shape = (n_sel, self.height * ts, self.width * ts, 3)
+        width, height = self.width, self.height
+        if self.mixed and n_sel:
+            dims = {self._dims[g] for g in np.unique(self.group_of(np.arange(self.num_envs) if ids is None else ids))}
+            if len(dims) != 1:
+                raise ValueError('the envs of one render_grid call must share one grid size (got %s): render each size separately'
+                                 % sorted(dims))
+            width, height = dims.pop()
+        shape = (n_sel, height * ts, width * ts, 3)
         if out is None:
             out = torch.empty(shape, dtype=torch.uint8, device=self.device)
         _check(out, 'out', self.device, torch.uint8, shape)
@@ -311,6 +382,7 @@ class BabyAIVecEnv(object):
 
     def step_timed(self, actions):
         """bb_pool_step with CUDA events around each kernel -> (ms k_step, ms k_gen)."""
+        self._single_level('step_timed')
         a, b = C.c_float(), C.c_float()
         _lib.check(self.L.bb_pool_step_timed(self.h, _ptr(actions), actions.element_size(), _ptr(self.obs),
                                              _ptr(self.reward), _ptr(self.done), _ptr(self.direction),
@@ -327,6 +399,7 @@ class BabyAIVecEnv(object):
 
     def rollout_timed(self, actions, obs, reward, done, direction=None):
         """rollout() with CUDA events around the stepping kernel and the level refill -> (ms, ms)."""
+        self._single_level('rollout_timed')
         self._check_rollout(actions, obs, reward, done, direction)
         a, b = C.c_float(), C.c_float()
         _lib.check(self.L.bb_pool_rollout_timed(self.h, _ptr(actions), actions.shape[0], _ptr(obs), _ptr(reward), _ptr(done),
@@ -359,7 +432,9 @@ class BabyAIVecEnv(object):
         return [detokenize(tok[i]) for i in idx]
 
     def state(self, i):
-        grid = np.zeros((self.height, self.width), np.uint8)
+        """(grid uint8 [H, W] of the env's own level, hidden-state dict)"""
+        width, height = self._dims[int(self.group_of(int(i)))] if 0 <= int(i) < self.num_envs else (self.width, self.height)
+        grid = np.zeros((height, width), np.uint8)
         info = np.zeros(8, np.int32)
         _lib.check(self.L.bb_pool_get_state(self.h, i, grid.ctypes.data_as(C.c_void_p), info.ctypes.data_as(C.c_void_p)))
         return grid, dict(agent_x=int(info[0]), agent_y=int(info[1]), agent_dir=int(info[2]), carrying=int(info[3]),
@@ -406,16 +481,37 @@ class EnvHandle(object):
 
 
 class EnvList(list):
-    """What scripts/train_rl.py:53-60 builds: N seeded envs of one level."""
+    """What scripts/train_rl.py:53-60 builds: N seeded envs of one level -- or of several: `level` is then the list of
+    (level_name, count) groups, in env order.  Two lists concatenate with `+` into the list of both groups."""
 
     def __init__(self, level, seeds, device=0, pixel=False):
         self.level, self.seeds, self.device, self.pixel = level, list(seeds), device, bool(pixel)
         super().__init__(EnvHandle(self, i) for i in range(len(self.seeds)))
 
+    def level_counts(self):
+        """[(level_name, count), ...] in env order"""
+        return level_groups(self.level) or [(self.level, len(self))]
 
-def make_envs(level, num_envs, seed=1, device=0, pixel=False):
+    def __add__(self, other):
+        if not isinstance(other, EnvList):
+            return list(self) + list(other)
+        if other.device != self.device or other.pixel != self.pixel:
+            raise ValueError('only env lists on the same device and with the same observation wrapper concatenate')
+        return EnvList(self.level_counts() + other.level_counts(), self.seeds + other.seeds, self.device, self.pixel)
+
+
+def make_envs(level, num_envs=None, seed=1, device=0, pixel=False):
     """`env.seed(100 * seed + i)` for env i (scripts/train_rl.py:59); pixel=True: every env wrapped in
-    RGBImgPartialObsWrapper (train_rl.py:54-58, `'pixel' in args.arch`)."""
+    RGBImgPartialObsWrapper (train_rl.py:54-58, `'pixel' in args.arch`).  `level` may be a dict or a sequence of
+    (level_name, count) pairs, e.g. {'GoToLocal': 64, 'BossLevel': 64}: the envs of several levels in that order (a
+    multi-task list), i counting over the whole list; num_envs is then the sum of the counts or None."""
+    groups = level_groups(level)
+    if groups is not None:
+        total = sum(c for _, c in groups)
+        if num_envs is not None and int(num_envs) != total:
+            raise ValueError('num_envs (%d) is not the sum of the group sizes (%d)' % (num_envs, total))
+        num_envs = total
+        level = groups if len(groups) > 1 else groups[0][0]
     return EnvList(level, [100 * seed + i for i in range(num_envs)], device, pixel)
 
 
@@ -431,18 +527,25 @@ def RGBImgPartialObsWrapper(envs, tile_size=8):
 
 def _as_env_list(envs, need_seeds):
     """An EnvList as is.  A plain list of reference envs -- what `batch_evaluate` builds with gym.make before it
-    wraps them in ManyEnvs (evaluate.py:86-94) -- is accepted where the seeds arrive later through seed(): the level is
-    read from the reference's own class attribute (`level_name`, levelgen.py:492)."""
+    wraps them in ManyEnvs (evaluate.py:86-94) -- is accepted where the seeds arrive later through seed(): the level of
+    each env is read from the reference's own class attribute (`level_name`, levelgen.py:492), and maximal runs of one
+    level become the groups of a mixed pool, in list order."""
     if isinstance(envs, EnvList):
         return envs
     if need_seeds:
         raise TypeError('build the env list with babyai_b200.make_envs(): the seeds of gym envs cannot be read back')
-    first = envs[0]
-    first = getattr(first, 'unwrapped', first)
-    name = getattr(type(first), 'level_name', None)
-    if not isinstance(name, str):
-        raise TypeError('cannot tell the BabyAI level of %r; use babyai_b200.make_envs()' % (first,))
-    return EnvList(name, [0] * len(envs))
+    groups = []
+    for env in envs:
+        env = getattr(env, 'unwrapped', env)
+        name = getattr(type(env), 'level_name', None)
+        if not isinstance(name, str):
+            raise TypeError('cannot tell the BabyAI level of %r; use babyai_b200.make_envs()' % (env,))
+        if groups and groups[-1][0] == name:
+            groups[-1][1] += 1
+        else:
+            groups.append([name, 1])
+    groups = [tuple(g) for g in groups]
+    return EnvList(groups if len(groups) > 1 else groups[0][0], [0] * len(envs))
 
 
 class _HostVec(object):

@@ -92,6 +92,24 @@ typedef struct bb_pool bb_pool;
 int bb_pool_create(const bb_level_spec *spec, int32_t n_envs, int32_t device, bb_pool **out);
 int bb_pool_destroy(bb_pool *pool);
 
+/* Replaces: a list of gym envs of SEVERAL levels handed to ParallelEnv(envs) / ManyEnvs(envs) (penv.py:18-59,
+ * evaluate.py:58-81; the multi_env list of imitation.py:83-84,163-165,326-338; multi-task and curriculum training).  A MIXED
+ * pool of n_groups contiguous groups: group g holds envs [start_g, start_g + counts[g]) (start_0 = 0, in list order) of level
+ * specs[g]; a spec may appear in several groups.  Each group is an ordinary pool of its level -- its own state layout, level
+ * ring, generation schedule and kernels -- whose rows of every buffer are [start_g, start_g + counts[g]), so a mixed pool
+ * computes exactly what its groups compute as separate pools with the same seeds (default seeds: 0 .. counts[g] - 1 in each
+ * group).  The handle is a bb_pool: every entry point below takes it (the exceptions are listed there).  The mission tokens of
+ * all groups are one int16 [N][L] array, L the largest max_tokens of the groups (shorter missions are zero-padded).  Rollout
+ * and step outputs keep the UBLKCP bulk-store path where a group's rows start on a multiple of 16 envs and (rollout) N is
+ * one too: group sizes that are multiples of 32 keep it everywhere, other sizes are correct through plain stores.
+ * Counts >= 1, N <= INT32_MAX; n_groups = 1 is bb_pool_create. */
+int bb_pool_create_mixed(const bb_level_spec *specs, const int32_t *counts, int32_t n_groups, int32_t device, bb_pool **out);
+/* 1 for a pool of one level; group g's first env, env count and level spec (any pointer may be NULL). */
+int32_t bb_pool_num_groups(const bb_pool *pool);
+int bb_pool_group(const bb_pool *pool, int32_t g, int32_t *start, int32_t *count, bb_level_spec *spec_out);
+/* grid width / height of env `env` (on a mixed pool they differ between groups) */
+int bb_pool_env_dims(const bb_pool *pool, int32_t env, int32_t *w, int32_t *h);
+
 /* Replaces: env.seed(seed) per env (scripts/train_rl.py:59; ManyEnvs.seed
  * evaluate.py:64-65).  seeds_host[n_envs]; restarts each env's random stream. */
 int bb_pool_seed(bb_pool *pool, const uint64_t *seeds_host);
@@ -134,7 +152,10 @@ int bb_pool_reset_envs(bb_pool *pool, const int32_t *env_ids_host, const uint64_
  * the observation of the env's state after the call; no other row is written; the loaded envs' mission tokens are
  * rewritten.  Envs not listed keep their state, level rings and streams.  Counters are unchanged.
  * Both: arguments are checked before anything is enqueued, n_sel = 0 enqueues nothing; asynchronous and stream-ordered on
- * `stream` (the caller orders records_dev between streams); the host arrays are consumed before the call returns. */
+ * `stream` (the caller orders records_dev between streams); the host arrays are consumed before the call returns.
+ * Not on a mixed pool (an error, nothing enqueued; bb_pool_env_record_bytes returns 0): a record's layout tag is made of the
+ * grid size, token width and ring depth, not of the level, so a record of one group's level would load silently into an env
+ * of another level with the same layout. */
 int64_t bb_pool_env_record_bytes(const bb_pool *pool);
 int bb_pool_save_envs(bb_pool *pool, const int32_t *env_ids_host, int32_t n_sel, uint8_t *records_dev, void *stream);
 int bb_pool_load_envs(bb_pool *pool, const int32_t *env_ids_host, const int32_t *slots_host, int32_t n_sel,
@@ -167,7 +188,8 @@ int bb_pool_step_envs(bb_pool *pool, const int32_t *env_ids_host, int32_t n_sel,
                       uint8_t *obs_dev, float *reward_dev, uint8_t *done_dev, int8_t *dir_dev, void *stream);
 
 /* bb_pool_step on the pool's internal stream with CUDA events around each of its
- * two kernels (measurement hook for bench.py's roofline line; synchronises). */
+ * two kernels (measurement hook for bench.py's roofline line; synchronises).  Not on a mixed pool (one pair of times per
+ * level). */
 int bb_pool_step_timed(bb_pool *pool, const void *actions_dev, int32_t action_bytes,
                        uint8_t *obs_dev, float *reward_dev, uint8_t *done_dev, int8_t *dir_dev,
                        float *ms_step_kernel, float *ms_gen_kernel);
@@ -179,27 +201,30 @@ int bb_pool_step_timed(bb_pool *pool, const void *actions_dev, int32_t action_by
  * bb_pool_step.  Grids up to 22 x 22 with a ring of pre-generated levels deep enough
  * (>= 3 T): ONE persistent kernel keeps the env state in shared memory for the T steps
  * (single-room levels: level generation runs inside it too); otherwise one CUDA graph
- * of T step launches. */
+ * of T step launches.  Mixed pool: each group runs on an internal stream of its own, forked from `stream` and joined back
+ * into it, so the groups' kernels share the GPU; every buffer keeps the row stride N between steps. */
 int bb_pool_rollout(bb_pool *pool, const int8_t *actions_dev, int32_t T,
                     uint8_t *obs_dev, float *reward_dev, uint8_t *done_dev, int8_t *dir_dev, void *stream);
 
 /* bb_pool_rollout on the pool's internal stream with CUDA events around the stepping kernel and around the
  * level refill (measurement hook for bench.py's roofline line; synchronises).  Times are 0 when the call
- * took the per-step-graph path. */
+ * took the per-step-graph path.  Not on a mixed pool. */
 int bb_pool_rollout_timed(bb_pool *pool, const int8_t *actions_dev, int32_t T,
                           uint8_t *obs_dev, float *reward_dev, uint8_t *done_dev, int8_t *dir_dev,
                           float *ms_rollout_kernel, float *ms_refill);
 
 /* Same as bb_pool_step but with HOST buffers (what ParallelEnv.step hands
  * back to BaseAlgo.collect_experiences, rl/algos/base.py:144): copies actions
- * host->device, steps, copies obs/reward/done/dir device->host, synchronises. */
+ * host->device, steps, copies obs/reward/done/dir device->host, synchronises
+ * (a mixed pool: every group is enqueued first, then one synchronisation). */
 int bb_pool_step_host(bb_pool *pool, const int8_t *actions_host,
                       uint8_t *obs_host, float *reward_host, uint8_t *done_host, int8_t *dir_host);
 int bb_pool_reset_host(bb_pool *pool, uint8_t *obs_host, int8_t *dir_host);
 
 /* The learner's step (BaseAlgo.collect_experiences, rl/algos/base.py:131-188, with the observations resident on the
  * device): actions from a HOST buffer (base.py:144 hands numpy), observation (and optionally direction) into DEVICE
- * buffers on `stream`, reward / done into HOST buffers (base.py:158-179 reads them there); synchronises `stream`. */
+ * buffers on `stream`, reward / done into HOST buffers (base.py:158-179 reads them there); synchronises `stream` (once, after
+ * every group of a mixed pool). */
 int bb_pool_step_learner(bb_pool *pool, const int8_t *actions_host, uint8_t *obs_dev, float *reward_host,
                          uint8_t *done_host, int8_t *dir_dev, void *stream);
 
@@ -222,7 +247,7 @@ int bb_rgb_tiles(uint8_t *tiles_host);
  * NULL = every env in order (n_sel must then be n_envs).  tile_size 1..64.  rgb_dev: uint8 [n_sel][H*ts][W*ts][3],
  * 16-byte aligned.  Stream-ordered after the work already on `stream`, no synchronisation (the table of a tile size is
  * rasterised on the host and uploaded the first time that size is rendered); arguments are checked before anything is
- * launched. */
+ * launched.  On a mixed pool the selected envs must share one grid size (H, W of bb_pool_env_dims); an error otherwise. */
 int bb_pool_render_grid(bb_pool *pool, const int32_t *env_ids_host, int32_t n_sel, int32_t tile_size, int32_t highlight,
                         uint8_t *rgb_dev, void *stream);
 /* The full-grid tile table of one tile size (host, no GPU): uint8 [2][5][43][ts][ts][3] indexed by highlight, agent (0 none,
@@ -238,15 +263,15 @@ int32_t bb_vocab_size(void);
 const char *bb_vocab_word(int32_t id);   /* id 1..bb_vocab_size(); 0 = pad -> "" */
 
 /* Introspection for parity tests: one env's hidden state copied to host.
- * grid_host: uint8[height*width], cell = type | color<<3 | state<<6 (empty 0x01);
+ * grid_host: uint8[height*width] of the env's own grid (bb_pool_env_dims), cell = type | color<<3 | state<<6 (empty 0x01);
  * info_host: int32[8] = agent_x, agent_y, agent_dir, carrying cell byte (0 none),
  * step_count, max_steps, rng draws (low 31 bits), generation attempts. */
 int bb_pool_get_state(bb_pool *pool, int32_t env, uint8_t *grid_host, int32_t *info_host);
-int32_t bb_pool_width(const bb_pool *pool);
+int32_t bb_pool_width(const bb_pool *pool);      /* a mixed pool: the largest of its groups */
 int32_t bb_pool_height(const bb_pool *pool);
 int32_t bb_pool_num_envs(const bb_pool *pool);
 
-/* Counters since creation, summed on the device: [0] env-steps, [1] episodes
+/* Counters since creation, summed on the device (and over the groups of a mixed pool): [0] env-steps, [1] episodes
  * ended, [2] episodes ended in success, [3] internal errors (must stay 0).
  * (Multi-GPU runs all-gather these -- the only collective on this path.) */
 int bb_pool_counters(bb_pool *pool, int64_t *out4_host);
