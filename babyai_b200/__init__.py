@@ -14,6 +14,7 @@ from .levels import LEVELS, VOCAB, detokenize, level_spec  # noqa: F401
 def __getattr__(name):
     # vecenv imports torch and loads the CUDA library: keep `import babyai_b200` light
     if name in ('BabyAIVecEnv', 'ParallelEnv', 'ManyEnvs', 'make_envs', 'EnvList', 'preprocess_obss', 'RGBImgPartialObsWrapper',
+                'FullyObsWrapper', 'RGBImgObsWrapper',
                 'MODE_AUTORESET', 'MODE_FREEZE'):
         from . import vecenv
         return getattr(vecenv, name)

@@ -12,6 +12,7 @@
 //   k_save_envs, k_load_envs, k_observe8  bb_pool_save_envs / bb_pool_load_envs: env records out of and into the pool (env_record.cuh).
 //   k_step8_sel   bb_pool_step_envs: one step of the envs of an id list, eight lanes per environment (step8_sel.cuh).
 //   k_render_rgb, k_render_grid  pictures: the partial view of an observation, and the full grid of an env's current state.
+//   k_full_obs    bb_pool_full_obs: the fully observable observation (FullyObsWrapper) of the envs of an id list.
 // Levels depend only on the env's random stream, never on actions, so generating episodes k+1 .. k+D while episode k
 // is being played is equivalent to generating them at reset time: every env owns a ring of D pre-generated levels.
 // The per-environment logic (step, verifier, observation, generators) is env_logic.cuh; DESIGN.md section 4 has the
@@ -40,6 +41,7 @@
 #include <type_traits>
 #include "rgb_tiles.h"
 #include "grid_render.cuh"
+#include "full_obs.cuh"
 
 using namespace bb;
 
@@ -495,6 +497,35 @@ k_render_grid(const LevelParams lp, const PoolPtrs P, const Sel sel, const int n
             if (j >= ppr) { j -= ppr; ty++; }
             if (ty >= ts) { ty -= ts; cyw += W; }
         }
+    }
+}
+
+// k_full_obs -- FullyObsWrapper observations of selected envs, uint8[n_sel][W][H][3] (full_obs.cuh).  A frame is 3 W H
+// bytes (63 for KeyCorridorS3R1, 192 for GoToLocal, 1 452 for BossLevel): a CTA per frame would leave most threads idle, so
+// one warp handles one env at a time (grid-stride over the selection, selections as k_render_grid's):
+//   1. the lanes copy the env's GT cells, without the row padding, into the warp's slice of shared memory (the hidden cell of
+//      a PutNext*Carrying episode at step 0 as empty);
+//   2. the lanes write the frame as aligned 32-bit words, consecutive lanes consecutive words (full_obs_store); frame k starts
+//      at byte k 3 W H, so the up to three bytes before its first word boundary and after its last one are stored singly.
+constexpr int FO_THREADS = 256, FO_WARPS = FO_THREADS / 32, FO_BLOCKS_PER_SM = 8;
+constexpr int FO_STAGE = (FO_CELLS + 15) / 16 * 16;
+
+template <class Sel>
+__global__ void __launch_bounds__(FO_THREADS)
+k_full_obs(const LevelParams lp, const PoolPtrs P, const Sel sel, const int n_sel, uint8_t *__restrict__ out)
+{
+    __shared__ __align__(16) uint8_t s_cells[FO_WARPS][FO_STAGE];
+    const int lane = threadIdx.x & 31;
+    uint8_t *cells = s_cells[threadIdx.x >> 5];
+    const int F = 3 * lp.W * lp.H;
+    for (int k = blockIdx.x * FO_WARPS + (threadIdx.x >> 5); k < n_sel; k += gridDim.x * FO_WARPS) {
+        const int env = sel.env(k);
+        const uint8_t *grid = P.grid + (size_t)env * lp.cells_pad;
+        const FullObsPose e = full_obs_pose(lp, P.hot[env], P.obj[env], P.ins[env]);
+        __syncwarp();                              // every lane is done with the previous env's cells
+        full_obs_stage(lp, grid, e, cells, lane, 32);
+        __syncwarp();
+        full_obs_store(e, cells, F, out + (size_t)k * F, lane, 32);
     }
 }
 
@@ -965,6 +996,26 @@ static void launch_render_grid_ts(bb_pool *p, const int32_t *ids, int32_t n_sel,
     else launch_render_grid<1>(p, ids, n_sel, ts, hl, rgb, st, lut);
 }
 
+static void launch_full_obs(bb_pool *p, const int32_t *ids, int32_t n_sel, uint8_t *out, cudaStream_t st)
+{
+    const size_t frame = (size_t)3 * p->lp.W * p->lp.H;
+    const int cap = p->sm_count * FO_BLOCKS_PER_SM;
+    auto blocks = [cap](int m) { const int b = (m + FO_WARPS - 1) / FO_WARPS; return b < cap ? b : cap; };
+    if (!ids) {
+        const RgRange r = { 0 };
+        k_full_obs<RgRange><<<blocks(n_sel), FO_THREADS, 0, st>>>(p->lp, p->P, r, n_sel, out);
+        p->launches++;
+        return;
+    }
+    RgList l;
+    for (int32_t k0 = 0; k0 < n_sel; k0 += RG_IDS) {
+        const int m = n_sel - k0 < RG_IDS ? n_sel - k0 : RG_IDS;
+        memcpy(l.id, ids + k0, (size_t)m * sizeof(int32_t));
+        k_full_obs<RgList><<<blocks(m), FO_THREADS, 0, st>>>(p->lp, p->P, l, m, out + (size_t)k0 * frame);
+        p->launches++;
+    }
+}
+
 // ---- mixed pools (bb_pool_create_mixed; DESIGN.md section 4.11) ----------------------------------------------------------
 // Every entry point dispatches to the groups at its top, after the checks that do not depend on the level.  A whole-pool call
 // calls each group with the caller's pointers offset by the group's first row; an id-list call makes one call per maximal run of
@@ -1024,21 +1075,47 @@ static int mixed_step(bb_pool *p, const void *actions, int32_t action_bytes, uin
     return 0;
 }
 
+// the grid size every env of an id list (n_sel >= 1, in range) shares, for the calls whose output rows are frames of one size
+static const LevelParams *mixed_one_size(const bb_pool *p, const int32_t *ids, int32_t n_sel, const char *what)
+{
+    const LevelParams &l0 = p->groups[group_of(p, ids[0])]->lp;
+    for (int32_t k = 1; k < n_sel; k++) {
+        const LevelParams &l = p->groups[group_of(p, ids[k])]->lp;
+        if (l.W != l0.W || l.H != l0.H) {
+            fail("the envs of one %s call must share one grid size (on a mixed pool: one call per size)", what);
+            return nullptr;
+        }
+    }
+    return &l0;
+}
+
 static int mixed_render_grid(bb_pool *p, const int32_t *ids, int32_t n_sel, int ts, int hl, uint8_t *rgb, cudaStream_t st)
 {
     std::vector<int32_t> all;
     if (!ids) { all.resize((size_t)n_sel); for (int32_t k = 0; k < n_sel; k++) all[k] = k; ids = all.data(); }
-    const LevelParams &l0 = p->groups[group_of(p, ids[0])]->lp;
-    for (int32_t k = 1; k < n_sel; k++) {
-        const LevelParams &l = p->groups[group_of(p, ids[k])]->lp;
-        if (l.W != l0.W || l.H != l0.H) return fail("the envs of one render_grid call must share one grid size (on a mixed pool: one call per size)");
-    }
-    const size_t frame = (size_t)l0.H * l0.W * ts * ts * 3;
+    const LevelParams *l0 = mixed_one_size(p, ids, n_sel, "render_grid");
+    if (!l0) return 1;
+    const size_t frame = (size_t)l0->H * l0->W * ts * ts * 3;
     return for_each_run(p, ids, n_sel, [&](int g, int32_t k0, int32_t m, const int32_t *loc) {
         bb_pool *c = p->groups[g];
         const uint8_t *lut = nullptr;
         if (grid_table(c, ts, &lut) || order_after_last(c, st)) return 1;
         launch_render_grid_ts(c, loc, m, ts, hl, rgb + (size_t)k0 * frame, st, lut);
+        return 0;
+    });
+}
+
+static int mixed_full_obs(bb_pool *p, const int32_t *ids, int32_t n_sel, uint8_t *out, cudaStream_t st)
+{
+    std::vector<int32_t> all;
+    if (!ids) { all.resize((size_t)n_sel); for (int32_t k = 0; k < n_sel; k++) all[k] = k; ids = all.data(); }
+    const LevelParams *l0 = mixed_one_size(p, ids, n_sel, "full_obs");
+    if (!l0) return 1;
+    const size_t frame = (size_t)3 * l0->W * l0->H;
+    return for_each_run(p, ids, n_sel, [&](int g, int32_t k0, int32_t m, const int32_t *loc) {
+        bb_pool *c = p->groups[g];
+        if (order_after_last(c, st)) return 1;
+        launch_full_obs(c, loc, m, out + (size_t)k0 * frame, st);
         return 0;
     });
 }
@@ -1932,6 +2009,26 @@ int bb_pool_render_grid(bb_pool *p, const int32_t *env_ids_host, int32_t n_sel, 
     if (n_sel == 0) return 0;
     if (order_after_last(p, st)) return 1;
     launch_render_grid_ts(p, env_ids_host, n_sel, tile_size, hl, rgb_dev, st, lut);
+    CU(cudaGetLastError());
+    return 0;
+}
+
+int bb_pool_full_obs(bb_pool *p, const int32_t *env_ids_host, int32_t n_sel, uint8_t *out_dev, void *stream)
+{
+    if (!p || n_sel < 0 || (n_sel > 0 && !out_dev)) return fail("bad arguments");
+    if (!env_ids_host && n_sel != p->n) return fail("env_ids_host = NULL observes every env: n_sel must equal n_envs");
+    if (env_ids_host)
+        for (int32_t k = 0; k < n_sel; k++)
+            if (env_ids_host[k] < 0 || env_ids_host[k] >= p->n) return fail("env id out of range [0, n_envs)");
+    if (n_sel == 0) return 0;
+    CU(cudaSetDevice(p->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (is_mixed(p)) {
+        if (mixed_full_obs(p, env_ids_host, n_sel, out_dev, st)) return 1;
+    } else {
+        if (order_after_last(p, st)) return 1;
+        launch_full_obs(p, env_ids_host, n_sel, out_dev, st);
+    }
     CU(cudaGetLastError());
     return 0;
 }

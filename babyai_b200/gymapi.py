@@ -17,7 +17,7 @@ from enum import IntEnum
 import numpy as np
 
 from .levels import LEVELS
-from .vecenv import EnvList, ManyEnvs, _spaces
+from .vecenv import EnvList, ManyEnvs, _spaces, grid_dims
 
 
 class Actions(IntEnum):
@@ -29,6 +29,27 @@ class Actions(IntEnum):
     drop = 4
     toggle = 5
     done = 6
+
+
+class Grid(object):
+    """MiniGridEnv.grid as far as gym_minigrid's FullyObsWrapper reads it (wrappers.py): `encode()` of the env's current
+    state, made on the device by bb_pool_full_obs."""
+
+    def __init__(self, env):
+        self._env = env
+        self.width, self.height = env.width, env.height
+
+    def encode(self, vis_mask=None):
+        """Grid.encode(): uint8[W, H, 3] of (type, color, state) per cell, x-major; the agent is not part of the grid"""
+        if vis_mask is not None:
+            raise NotImplementedError('Grid.encode(vis_mask): the pool encodes whole grids')
+        pool = self._env._vec.pool
+        img = pool.full_obs([0])[0].cpu().numpy()
+        grid, s = pool.state(0)
+        x, y = s['agent_x'], s['agent_y']
+        b = int(grid[y, x])                               # what the agent stands on: empty, or an open door
+        img[x, y] = (b & 7, (b >> 3) & 7, b >> 6)
+        return img
 
 
 def _level_of(name):
@@ -56,6 +77,8 @@ class SingleEnv(object):
             seed = int.from_bytes(os.urandom(4), 'little')
         self._vec = ManyEnvs(EnvList(self.level_name, [seed], device), pool=pool)
         self.mission = None
+        self.width, self.height = grid_dims([(self.level_name, 1)])     # MiniGridEnv.width / height
+        self.grid = Grid(self)
 
     @property
     def unwrapped(self):

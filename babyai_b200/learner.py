@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from .levels import VOCAB, detokenize
-from .vecenv import MODE_AUTORESET, MODE_FREEZE, BabyAIVecEnv, _as_env_list, _spaces
+from .vecenv import MODE_AUTORESET, MODE_FREEZE, BabyAIVecEnv, _as_env_list, _spaces, full_image
 
 
 class ObsTensors(object):
@@ -173,7 +173,8 @@ class DeviceParallelEnv(object):
     with BabyAIVecEnv's tensor interface (the GPU-less suite passes the host build of the kernel logic).
     `fused_io` (default on; BB_LEARNER_FUSED_IO=0 switches it off) steps through bb_pool_step_learner -- actions, reward and
     done travel over mapped page-locked memory inside the one step call instead of as three separate tensor copies
-    A list wrapped in RGBImgPartialObsWrapper (`make_envs(..., pixel=True)`) yields 56x56x3 pictures rendered on the device."""
+    A list wrapped in RGBImgPartialObsWrapper (`make_envs(..., pixel=True)`) yields 56x56x3 pictures rendered on the device;
+    one wrapped in FullyObsWrapper / RGBImgObsWrapper yields the full grid's encoding / picture of every env's current state."""
 
     MODE = MODE_AUTORESET
 
@@ -181,7 +182,8 @@ class DeviceParallelEnv(object):
         envs = _as_env_list(envs, need_seeds=(self.MODE == MODE_AUTORESET))
         self.envs = envs
         self.pixel = bool(getattr(envs, 'pixel', False))      # RGBImgPartialObsWrapper'd list: batches carry uint8[N, 56, 56, 3]
-        self.observation_space, self.action_space = _spaces(self.pixel)
+        self.full, self.tile_size = envs.full, envs.tile_size
+        self.observation_space, self.action_space = _spaces(self.pixel, envs.image_shape())
         self.pool = pool if pool is not None else BabyAIVecEnv(envs.level, len(envs), seeds=envs.seeds,
                                                                device=envs.device, mode=self.MODE)
         self._tokens = None
@@ -197,7 +199,10 @@ class DeviceParallelEnv(object):
         return ObsBatch(self._pix(image), self._tokens, self.pool.direction.clone())
 
     def _pix(self, image):
-        """pixel mode: the 7x7x3 observation the step kernel wrote -> the 56x56x3 picture (one HBM-bound kernel)"""
+        """pixel mode: the 7x7x3 observation the step kernel wrote -> the 56x56x3 picture (one HBM-bound kernel); a fully
+        observable list: the image of every env's current state instead"""
+        if self.full is not None:
+            return full_image(self.pool, self.full, self.tile_size)
         return self.pool.render_rgb(image) if self.pixel else image
 
     def _new_image(self):
@@ -236,7 +241,15 @@ class DeviceParallelEnv(object):
         """the batch `obs` with the rows of envs env_ids (None: every env) rewritten by `write(obs=, direction=)`, a pool
         call that writes those rows of raw observations and directions, and with the pool's current missions"""
         img, dire = obs.image, obs.direction.clone()
-        if self.pixel:
+        if self.full is not None:
+            write(obs=self._new_image(), direction=dire)
+            img = img.clone()
+            if env_ids is None:
+                img.copy_(full_image(self.pool, self.full, self.tile_size))
+            else:
+                ids = np.asarray(env_ids, dtype=np.int64)
+                img[torch.as_tensor(ids, device=self.pool.device)] = full_image(self.pool, self.full, self.tile_size, ids)
+        elif self.pixel:
             raw = self._new_image()
             write(obs=raw, direction=dire)
             idx = slice(None) if env_ids is None else torch.as_tensor(np.asarray(env_ids, dtype=np.int64), device=self.pool.device)

@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(HERE, 'libbabyai_b200.so')
 SYMBOLS = [
     'bb_pool_create', 'bb_pool_create_mixed', 'bb_pool_num_groups', 'bb_pool_group', 'bb_pool_env_dims', 'bb_pool_destroy', 'bb_pool_seed', 'bb_pool_set_mode', 'bb_pool_reset', 'bb_pool_reset_envs', 'bb_pool_env_record_bytes',
     'bb_pool_save_envs', 'bb_pool_load_envs', 'bb_pool_step', 'bb_pool_step_envs',
-    'bb_pool_step_timed', 'bb_pool_rollout', 'bb_pool_rollout_timed', 'bb_pool_step_host', 'bb_pool_reset_host', 'bb_pool_step_learner', 'bb_pool_mission_tokens', 'bb_pool_render_rgb', 'bb_rgb_tiles', 'bb_pool_render_grid', 'bb_grid_tiles', 'bb_vocab_size',
+    'bb_pool_step_timed', 'bb_pool_rollout', 'bb_pool_rollout_timed', 'bb_pool_step_host', 'bb_pool_reset_host', 'bb_pool_step_learner', 'bb_pool_mission_tokens', 'bb_pool_render_rgb', 'bb_rgb_tiles', 'bb_pool_render_grid', 'bb_grid_tiles', 'bb_pool_full_obs', 'bb_vocab_size',
     'bb_vocab_word', 'bb_pool_get_state', 'bb_pool_width', 'bb_pool_height', 'bb_pool_num_envs',
     'bb_pool_counters', 'bb_pool_launches', 'bb_last_error',
 ]
@@ -60,6 +60,7 @@ def load():
     L.bb_rgb_tiles.argtypes = [vp]
     L.bb_pool_render_grid.argtypes = [vp, vp, i32, i32, i32, vp, vp]
     L.bb_grid_tiles.argtypes = [i32, vp]
+    L.bb_pool_full_obs.argtypes = [vp, vp, i32, vp, vp]
     L.bb_pool_mission_tokens.argtypes = [vp, C.POINTER(vp), C.POINTER(i32)]
     L.bb_vocab_size.restype = i32
     L.bb_vocab_word.restype = C.c_char_p

@@ -365,13 +365,7 @@ class BabyAIVecEnv(object):
         if env_ids is not None:
             ids = self._env_ids(env_ids)
             n_sel = ids.size
-        width, height = self.width, self.height
-        if self.mixed and n_sel:
-            dims = {self._dims[g] for g in np.unique(self.group_of(np.arange(self.num_envs) if ids is None else ids))}
-            if len(dims) != 1:
-                raise ValueError('the envs of one render_grid call must share one grid size (got %s): render each size separately'
-                                 % sorted(dims))
-            width, height = dims.pop()
+        width, height = self._sel_dims(ids, n_sel, 'render_grid')
         shape = (n_sel, height * ts, width * ts, 3)
         if out is None:
             out = torch.empty(shape, dtype=torch.uint8, device=self.device)
@@ -379,6 +373,31 @@ class BabyAIVecEnv(object):
         _lib.check(self.L.bb_pool_render_grid(self.h, ids.ctypes.data_as(C.c_void_p) if ids is not None else None, n_sel, ts,
                                               1 if highlight else 0, _ptr(out), self._stream()))
         return out
+
+    def full_obs(self, env_ids=None, out=None):
+        """FullyObsWrapper.observation(obs)['image'] of the selected envs' CURRENT states (bb_pool_full_obs): grid.encode() of
+        the whole grid with the agent's cell (10, 0, agent_dir), uint8 [n_sel, W, H, 3] (x-major) on the device.  env_ids: ids
+        in [0, N) in any order, repeats allowed (default: every env in order).  On a mixed pool the selected envs must share one
+        grid size."""
+        ids = None if env_ids is None else self._env_ids(env_ids)
+        n_sel = self.num_envs if ids is None else ids.size
+        width, height = self._sel_dims(ids, n_sel, 'full_obs')
+        shape = (n_sel, width, height, 3)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.uint8, device=self.device)
+        _check(out, 'out', self.device, torch.uint8, shape)
+        _lib.check(self.L.bb_pool_full_obs(self.h, ids.ctypes.data_as(C.c_void_p) if ids is not None else None, n_sel,
+                                           _ptr(out), self._stream()))
+        return out
+
+    def _sel_dims(self, ids, n_sel, what):
+        """(width, height) every selected env shares; on a mixed pool a ValueError when they differ"""
+        if not (self.mixed and n_sel):
+            return self.width, self.height
+        dims = {self._dims[g] for g in np.unique(self.group_of(np.arange(self.num_envs) if ids is None else ids))}
+        if len(dims) != 1:
+            raise ValueError('the envs of one %s call must share one grid size (got %s): call once per size' % (what, sorted(dims)))
+        return dims.pop()
 
     def step_timed(self, actions):
         """bb_pool_step with CUDA events around each kernel -> (ms k_step, ms k_gen)."""
@@ -456,11 +475,12 @@ class _Space(object):
     pass
 
 
-def _spaces(pixel=False):
+def _spaces(pixel=False, image_shape=None):
     """observation_space / action_space with the attributes the reference reads
-    (utils/format.py:124-126: .spaces['image'].shape/.high; train_rl.py:96: action_space.n)."""
+    (utils/format.py:124-126: .spaces['image'].shape/.high; train_rl.py:96: action_space.n).  image_shape: the image of a
+    fully observable list (EnvList.image_shape)."""
     img = _Space()
-    img.shape = (56, 56, 3) if pixel else (7, 7, 3)
+    img.shape = image_shape if image_shape is not None else (56, 56, 3) if pixel else (7, 7, 3)
     img.low = np.zeros(img.shape, np.uint8)
     img.high = np.full(img.shape, 255, np.uint8)
     img.dtype = np.dtype('uint8')
@@ -477,27 +497,58 @@ class EnvHandle(object):
     def __init__(self, pool_spec, index):
         self.pool_spec = pool_spec
         self.index = index
-        self.observation_space, self.action_space = _spaces(getattr(pool_spec, 'pixel', False))
+        self.observation_space, self.action_space = _spaces(getattr(pool_spec, 'pixel', False), pool_spec.image_shape())
 
 
 class EnvList(list):
     """What scripts/train_rl.py:53-60 builds: N seeded envs of one level -- or of several: `level` is then the list of
-    (level_name, count) groups, in env order.  Two lists concatenate with `+` into the list of both groups."""
+    (level_name, count) groups, in env order.  Two lists concatenate with `+` into the list of both groups.
+    `full`: None (the 7x7 view, or its pictures with `pixel`), 'grid' (FullyObsWrapper) or 'rgb' (RGBImgObsWrapper at
+    `tile_size`)."""
 
-    def __init__(self, level, seeds, device=0, pixel=False):
+    def __init__(self, level, seeds, device=0, pixel=False, full=None, tile_size=8):
         self.level, self.seeds, self.device, self.pixel = level, list(seeds), device, bool(pixel)
+        self.full, self.tile_size = full, int(tile_size)
         super().__init__(EnvHandle(self, i) for i in range(len(self.seeds)))
 
     def level_counts(self):
         """[(level_name, count), ...] in env order"""
         return level_groups(self.level) or [(self.level, len(self))]
 
+    def wrapper(self):
+        """what a batch of this list's observations is made of"""
+        return (self.pixel, self.full, self.tile_size if self.full == 'rgb' else None)
+
+    def image_shape(self):
+        """obs['image'].shape of a fully observable list: FullyObsWrapper (W, H, 3); RGBImgObsWrapper (H ts, W ts, 3), the
+        shape of the array MiniGridEnv.render returns (gym_minigrid declares (W ts, H ts, 3)); None for the 7x7 view"""
+        if self.full is None:
+            return None
+        width, height = grid_dims(self.level_counts())
+        return (width, height, 3) if self.full == 'grid' else (height * self.tile_size, width * self.tile_size, 3)
+
     def __add__(self, other):
         if not isinstance(other, EnvList):
             return list(self) + list(other)
-        if other.device != self.device or other.pixel != self.pixel:
+        if other.device != self.device or other.wrapper() != self.wrapper():
             raise ValueError('only env lists on the same device and with the same observation wrapper concatenate')
-        return EnvList(self.level_counts() + other.level_counts(), self.seeds + other.seeds, self.device, self.pixel)
+        out = EnvList(self.level_counts() + other.level_counts(), self.seeds + other.seeds, self.device, self.pixel,
+                      self.full, self.tile_size)
+        out.image_shape()                                  # a fully observable list of two grid sizes fails here
+        return out
+
+
+def grid_dims(groups):
+    """(width, height) of the grids of every level of [(level_name, count), ...] (RoomGrid: (room_size - 1) * num_cols + 1
+    by (room_size - 1) * num_rows + 1); a ValueError when the levels' grids differ in size"""
+    dims = set()
+    for name, _ in groups:
+        s = level_spec(name)
+        dims.add(((s.room_size - 1) * s.num_cols + 1, (s.room_size - 1) * s.num_rows + 1))
+    if len(dims) != 1:
+        raise ValueError('a fully observable env list needs one grid size, got %s: wrap the lists of each size separately'
+                         % sorted(dims))
+    return dims.pop()
 
 
 def make_envs(level, num_envs=None, seed=1, device=0, pixel=False):
@@ -523,6 +574,38 @@ def RGBImgPartialObsWrapper(envs, tile_size=8):
     if not isinstance(envs, EnvList):
         raise TypeError('wrap the list make_envs() built')
     return EnvList(envs.level, envs.seeds, envs.device, pixel=True)
+
+
+def _wrap_full(envs, full, tile_size):
+    if not isinstance(envs, EnvList):
+        raise TypeError('wrap the list make_envs() built')
+    if envs.wrapper() != (False, None, None):
+        raise ValueError('the list is already wrapped: its envs have one observation wrapper')
+    out = EnvList(envs.level, envs.seeds, envs.device, full=full, tile_size=tile_size)
+    out.image_shape()                                      # one grid size
+    return out
+
+
+def FullyObsWrapper(envs):
+    """gym_minigrid.wrappers.FullyObsWrapper for a whole env list: the pool's facades then return obs['image'] as
+    grid.encode() of the whole grid, uint8[W, H, 3] with the agent's cell (10, 0, agent_dir), made on the device by
+    bb_pool_full_obs, and obs dicts {'mission', 'image'}.  The levels of the list must share one grid size."""
+    return _wrap_full(envs, 'grid', 8)
+
+
+def RGBImgObsWrapper(envs, tile_size=8):
+    """gym_minigrid.wrappers.RGBImgObsWrapper for a whole env list: obs['image'] is env.render('rgb_array', highlight=False,
+    tile_size), uint8[H * tile_size, W * tile_size, 3], drawn on the device by bb_pool_render_grid (tile sizes 1..64)."""
+    if isinstance(tile_size, bool) or int(tile_size) != tile_size or not 1 <= tile_size <= 64:
+        raise ValueError('tile_size must be in 1..64 (got %r)' % (tile_size,))
+    return _wrap_full(envs, 'rgb', int(tile_size))
+
+
+def full_image(pool, full, tile_size, env_ids=None):
+    """the fully observable images of a pool's envs (default: all): FullyObsWrapper ('grid') or RGBImgObsWrapper ('rgb')"""
+    if full == 'grid':
+        return pool.full_obs(env_ids)
+    return pool.render_grid(env_ids, tile_size=tile_size, highlight=False)
 
 
 def _as_env_list(envs, need_seeds):
@@ -555,7 +638,8 @@ class _HostVec(object):
         envs = _as_env_list(envs, need_seeds=(mode == MODE_AUTORESET))
         self.envs = envs
         self.pixel = bool(getattr(envs, 'pixel', False))
-        self.observation_space, self.action_space = _spaces(self.pixel)
+        self.full, self.tile_size = envs.full, envs.tile_size
+        self.observation_space, self.action_space = _spaces(self.pixel, envs.image_shape())
         self.pool = pool if pool is not None else BabyAIVecEnv(envs.level, len(envs), seeds=envs.seeds, device=envs.device, mode=mode)
         n = len(envs)
         # page-locked host buffers: bb_pool_step_host DMAs straight into them
@@ -573,6 +657,9 @@ class _HostVec(object):
             if len(idx):
                 for i, m in zip(idx, self.pool.missions(idx)):
                     self._missions[i] = m
+        if self.full is not None:    # FullyObsWrapper / RGBImgObsWrapper.observation: {'mission', 'image'} of the current state
+            img = full_image(self.pool, self.full, self.tile_size).cpu().numpy()
+            return [{'image': img[i], 'mission': self._missions[i]} for i in range(len(self.envs))]
         if self.pixel:               # RGBImgPartialObsWrapper.observation: {'mission', 'image' uint8[56, 56, 3]} (no 'direction')
             dev = self.pool.device
             img = self.pool.render_rgb(torch.as_tensor(self._obs).to(dev)).cpu().numpy()

@@ -255,6 +255,15 @@ int bb_pool_render_grid(bb_pool *pool, const int32_t *env_ids_host, int32_t n_se
  * 25 + 6 state + color for doors).  For parity tests. */
 int bb_grid_tiles(int32_t tile_size, uint8_t *tiles_host);
 
+/* Replaces: gym_minigrid 1.0.x FullyObsWrapper.observation(obs)['image']: grid.encode() of each selected env's CURRENT
+ * state, uint8 [n_sel][W][H][3] in x-major order (row k of out_dev is env env_ids_host[k]), each cell (type, color, state) of
+ * OBJECT_TO_IDX / COLOR_TO_IDX / STATE_TO_IDX, an empty cell (1, 0, 0), and the agent's cell (10 = 'agent', 0 = 'red',
+ * agent_dir).  The carried object is not in the grid.  env_ids_host: n_sel ids in [0, n_envs), any order, repeats allowed;
+ * NULL = every env in order (n_sel must then be n_envs).  Any alignment of out_dev.  Stream-ordered after the work already on
+ * `stream`, no synchronisation; arguments are checked before anything is launched.  On a mixed pool the selected envs must
+ * share one grid size (W, H of bb_pool_env_dims); an error otherwise, with nothing launched. */
+int bb_pool_full_obs(bb_pool *pool, const int32_t *env_ids_host, int32_t n_sel, uint8_t *out_dev, void *stream);
+
 /* Replaces: obs['mission'] + InstructionsPreprocessor (utils/format.py:59-75).
  * Device pointer to int16 [n_envs][max_len] token ids of the current missions
  * (0 = pad, ids index bb_vocab_word); rewritten whenever an env is reset. */
